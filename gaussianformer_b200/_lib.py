@@ -20,7 +20,7 @@ GF_FLAG_MEAN_OUT_OF_GRID = 2
 GF_FLAG_RADIUS_LT_1 = 4
 GF_FLAG_GENERIC_PATH = 256
 
-DEBUG_EXPORTS = ("gf_debug_set_render_events", "gf_debug_gather_probe", "gf_debug_daf_forward_tma")   # include/gf_b200_debug.h: measurement hooks, not the drop-in boundary
+DEBUG_EXPORTS = ("gf_debug_set_render_events", "gf_debug_gather_probe")   # include/gf_b200_debug.h: measurement hooks, not the drop-in boundary
 EXPORTS = (
     "gf_abi_version", "gf_last_error", "gf_splat_supported_classes",
     "gf_splat_forward_workspace_bytes", "gf_splat_backward_workspace_bytes",
@@ -103,8 +103,6 @@ def lib():
         L.gf_splat_read_flags.argtypes = [c_void_p, c_void_p, POINTER(c_uint32)]
         L.gf_debug_set_render_events.argtypes = [c_void_p, c_void_p]
         L.gf_debug_gather_probe.argtypes = [c_void_p, c_void_p, ctypes.c_int64, c_int32, c_void_p, c_void_p]
-        L.gf_debug_daf_forward_tma.argtypes = [POINTER(DafDesc), c_void_p, POINTER(c_int32), POINTER(c_int32), c_void_p, c_void_p,
-                                               c_void_p, c_void_p]
         L.gf_splat_ce_partials.argtypes = [POINTER(SplatDesc)]
         L.gf_splat_ce_partials.restype = c_int
         L.gf_daf_forward.argtypes = [POINTER(DafDesc)] + [c_void_p] * 7

@@ -4,8 +4,6 @@
 #include <cstdio>
 #include <cstring>
 
-#include <cstdlib>
-
 #include "common.cuh"
 #include "gf_b200_debug.h"
 
@@ -36,8 +34,6 @@ int launch_backward(const gf_splat_desc &d, const gf_splat_inputs &in, const gf_
                     int num_sms, cudaStream_t stream);
 int render_ctas_per_sample(const gf_splat_desc &d);
 extern thread_local cudaEvent_t g_ev_before, g_ev_after;
-extern const int kSupportedClasses[];
-extern const int kNumSupportedClasses;
 
 struct DafParams;
 int launch_daf_forward(const gf_daf_desc &d, const float *feat, const int32_t *shape, const int32_t *start,
@@ -57,14 +53,6 @@ int launch_daf_fused_backward(const gf_daf_desc &d, int K, const float *feat, co
                               float *grad_loc, float *grad_logits, int num_sms, cudaStream_t stream);
 
 thread_local cudaEvent_t g_ev_before = nullptr, g_ev_after = nullptr;
-
-bool pdl_enabled() {
-    static const bool on = [] {
-        const char *e = getenv("GF_B200_PDL");
-        return !(e && e[0] == '0');
-    }();
-    return on;
-}
 
 static int num_sms_of_current_device(int *out) {
     static int cached[64];
@@ -95,10 +83,7 @@ static int check_desc(const gf_splat_desc *d) {
     GF_REQUIRE(d->batch >= 0 && d->batch <= 65535, GF_ERR_INVALID_ARG, "splat: batch=%d outside [0, 65535]", d->batch);
     GF_REQUIRE(static_cast<long long>(batch_of(*d)) * d->N * d->C < (1ll << 40), GF_ERR_UNSUPPORTED,
                "splat: batch x N x C too large");
-    bool ok = false;
-    for (int i = 0; i < kNumSupportedClasses; ++i) ok = ok || kSupportedClasses[i] == d->C;
-    GF_REQUIRE(ok, GF_ERR_UNSUPPORTED, "splat: class count C=%d is not compiled in", d->C);
-    return GF_OK;
+    return dispatch_classes(d->C, "splat", [](auto) { return GF_OK; });
 }
 
 static int check_inputs(const gf_splat_desc *d, const gf_splat_inputs *in) {
@@ -134,7 +119,7 @@ int gf_debug_set_render_events(void *before, void *after) {
 
 int gf_splat_supported_classes(int32_t *out, int cap) {
     int n = 0;
-    for (; n < kNumSupportedClasses && n < cap; ++n) out[n] = kSupportedClasses[n];
+    for (int c = kMinClasses; c <= kMaxClasses && n < cap; ++c) out[n++] = c;
     return n;
 }
 

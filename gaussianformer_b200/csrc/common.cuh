@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "gf_b200.h"
 
 namespace gf {
@@ -27,6 +29,20 @@ int cuda_fail(cudaError_t e, const char *what);
             return (code);               \
         }                                \
     } while (0)
+
+// The class counts C the splat kernels are compiled for.  dispatch_classes returns f(std::integral_constant<int, C>{})
+// for one of them; any other C is reported as `what`'s error.
+constexpr int kMinClasses = 16, kMaxClasses = 20;
+template <int CC = kMinClasses, class F>
+int dispatch_classes(int C, const char *what, F &&f) {
+    if constexpr (CC > kMaxClasses) {
+        set_error("%s: class count C=%d is not compiled in (supported: %d..%d)", what, C, kMinClasses, kMaxClasses);
+        return GF_ERR_UNSUPPORTED;
+    } else {
+        if (C == CC) return f(std::integral_constant<int, CC>{});
+        return dispatch_classes<CC + 1>(C, what, f);
+    }
+}
 
 // ---------------------------------------------------------------------------------------------
 // geometry of the splat pipeline
@@ -81,8 +97,7 @@ constexpr int kPackThreads = 64;   // small CTAs: ~400 of them cover the 132 SMs
 #ifdef __CUDACC__
 // Launches `kernel` so that it may become resident while the preceding kernel of the stream is still
 // running (programmatic stream serialization).  The kernel must call pdl_wait() before it touches
-// anything the preceding kernel writes.  GF_B200_PDL=0 falls back to plain stream order.
-bool pdl_enabled();
+// anything the preceding kernel writes.
 template <class... Params>
 cudaError_t launch_chained(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, const Params &...p) {
     cudaLaunchConfig_t cfg = {};
@@ -94,7 +109,7 @@ cudaError_t launch_chained(void (*kernel)(Params...), dim3 grid, dim3 block, siz
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, p...);
 }
 
@@ -168,6 +183,67 @@ __device__ __forceinline__ uint32_t lanemask_lt() {
     uint32_t m;
     asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m));
     return m;
+}
+
+// Phase A of the bin kernels (render_tile_kernel, backward_bin_kernel): the bin's ordered Gaussian list, resolved from
+// its supertile's list.  A bin entry is one Gaussian whose box overlaps the bin: .x holds the box clipped to the bin as
+// bit masks -- x columns in bits 0-7, y columns in bits 8-11, z levels in bits 16-31 -- and .y the Gaussian index.
+// All NT threads of the CTA test the candidates cand[cpos..ncand), the ascending list of supertile s (`lists`: [nsuper,
+// G]), fetching kPre rounds of NT before testing any (memory-level parallelism), and append the survivors to `list` in
+// the same order, compacted with ballots, until the candidates run out or another round might overflow SEG entries.
+// Advances cpos past the tested candidates and returns the number of entries.
+template <int NT, int kPre, int SEG>
+__device__ __forceinline__ int resolve_bin_list(const gf_splat_desc &d, const int32_t *lists, int s, int ncand, int &cpos,
+                                                const PackedBox *boxes, int binX0, int binY0, int binZ0, uint2 *list,
+                                                int (&warp_count)[2][NT / 32]) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int32_t *cand = lists + static_cast<size_t>(s) * d.G;
+    const uint32_t bX1 = min(binX0 + kBinX, d.H) - 1, bY1 = min(binY0 + kBinY, d.W) - 1, bZ1 = min(binZ0 + kBinZ, d.D) - 1;
+    int nlist = 0;
+    while (cpos < ncand && nlist + NT <= SEG) {
+        int gg[kPre];
+        uint4 bb[kPre];
+#pragma unroll
+        for (int u = 0; u < kPre; ++u) {
+            const int i = cpos + u * NT + tid;
+            gg[u] = i < ncand ? __ldg(cand + i) : -1;
+        }
+#pragma unroll
+        for (int u = 0; u < kPre; ++u)
+            bb[u] = gg[u] >= 0 ? __ldg(reinterpret_cast<const uint4 *>(boxes) + gg[u]) : make_uint4(1u, 1u, 1u, 1u);
+#pragma unroll
+        for (int u = 0; u < kPre; ++u) {
+            if (cpos >= ncand || nlist + NT > SEG) break;   // uniform
+            const uint4 b = bb[u];
+            const uint32_t x0 = b.x & 0xffffu, x1 = b.x >> 16, y0 = b.y & 0xffffu, y1 = b.y >> 16,
+                           z0 = b.z & 0xffffu, z1 = b.z >> 16;
+            const bool hit = gg[u] >= 0 && x0 <= bX1 && x1 >= static_cast<uint32_t>(binX0) && y0 <= bY1 &&
+                             y1 >= static_cast<uint32_t>(binY0) && z0 <= bZ1 && z1 >= static_cast<uint32_t>(binZ0) &&
+                             b.w == 0u;
+            const int rx0 = max(static_cast<int>(x0) - binX0, 0), rx1 = min(static_cast<int>(x1) - binX0, kBinX - 1);
+            const int ry0 = max(static_cast<int>(y0) - binY0, 0), ry1 = min(static_cast<int>(y1) - binY0, kBinY - 1);
+            const int rz0 = max(static_cast<int>(z0) - binZ0, 0), rz1 = min(static_cast<int>(z1) - binZ0, kBinZ - 1);
+            const uint32_t xm = ((2u << rx1) - 1u) & ~((1u << rx0) - 1u);
+            const uint32_t ym = ((2u << ry1) - 1u) & ~((1u << ry0) - 1u);
+            const uint32_t zm = ((2u << rz1) - 1u) & ~((1u << rz0) - 1u);
+            const uint2 entry = make_uint2(xm | (ym << 8) | (zm << 16), static_cast<uint32_t>(gg[u]));
+            const uint32_t ballot = __ballot_sync(0xffffffffu, hit);
+            if (lane == 0) warp_count[u & 1][warp] = __popc(ballot);
+            __syncthreads();
+            int off = nlist, total = 0;
+#pragma unroll
+            for (int k = 0; k < NT / 32; ++k) {
+                const int c = warp_count[u & 1][k];
+                if (k < warp) off += c;
+                total += c;
+            }
+            if (hit) list[off + __popc(ballot & lanemask_lt())] = entry;
+            nlist += total;
+            cpos += NT;
+        }
+        __syncthreads();
+    }
+    return nlist;
 }
 
 // ((v - origin) / cell) truncated toward zero, with the exact fp32 operation order of

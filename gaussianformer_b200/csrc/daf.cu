@@ -11,6 +11,7 @@
 //     weight gradients are reduced over the lanes of a group with shuffles and written by one
 //     lane, location gradients are reduced over the warp — no scalar atomic storms.
 #include "daf_pair.cuh"
+#include "gf_b200_debug.h"
 
 namespace gf {
 
@@ -53,36 +54,9 @@ __device__ __forceinline__ Bilinear bilinear_setup(float lx, float ly, int h, in
     return b;
 }
 
-template <int VEC> struct Vec;
-template <> struct Vec<4> {
-    using T = float4;
-    static __device__ __forceinline__ T zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
-    static __device__ __forceinline__ T load(const float *p) { return __ldg(reinterpret_cast<const float4 *>(p)); }
-    static __device__ __forceinline__ void fma(T &a, float s, const T &v) {
-        a.x = fmaf(s, v.x, a.x); a.y = fmaf(s, v.y, a.y); a.z = fmaf(s, v.z, a.z); a.w = fmaf(s, v.w, a.w);
-    }
-    static __device__ __forceinline__ float dot(const T &a, const T &b) { return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w; }
-    static __device__ __forceinline__ void store(float *p, const T &v) { *reinterpret_cast<float4 *>(p) = v; }
-    static __device__ __forceinline__ void atomic_add_scaled(float *p, float s, const T &v) {
-        atomicAdd(reinterpret_cast<float4 *>(p), make_float4(s * v.x, s * v.y, s * v.z, s * v.w));
-    }
-};
-template <> struct Vec<1> {
-    using T = float;
-    static __device__ __forceinline__ T zero() { return 0.f; }
-    static __device__ __forceinline__ T load(const float *p) { return __ldg(p); }
-    static __device__ __forceinline__ void fma(T &a, float s, const T &v) { a = fmaf(s, v, a); }
-    static __device__ __forceinline__ float dot(const T &a, const T &b) { return a * b; }
-    static __device__ __forceinline__ void store(float *p, const T &v) { *p = v; }
-    static __device__ __forceinline__ void atomic_add_scaled(float *p, float s, const T &v) { atomicAdd(p, s * v); }
-};
-
-// VEC = 4: C % 128 == 0 and (C/Gr)/4 a power of two <= 32 (a group is a run of whole lanes).
-// VEC = 1: any C, Gr.
-template <int VEC, bool BACKWARD>
+// Any C and Gr: a lane owns one channel per slice of 32 (shapes daf_fast_kernel does not take).
+template <bool BACKWARD>
 __global__ void __launch_bounds__(kDafThreads) daf_kernel(const DafParams p) {
-    using V = Vec<VEC>;
-    using T = typename V::T;
     const int lane = threadIdx.x & 31;
     const int C = p.d.num_embeds, M = p.d.num_cams, L = p.d.num_scale, Gr = p.d.num_groups, F = p.d.num_feat;
     const int gdim = C / Gr;
@@ -100,11 +74,11 @@ __global__ void __launch_bounds__(kDafThreads) daf_kernel(const DafParams p) {
     for (long long bp = static_cast<long long>(blockIdx.x) * (kDafThreads / 32) + (threadIdx.x >> 5); bp < npts; bp += warps) {
         const int b = static_cast<int>(bp / p.d.num_pts);
         const float *locp = p.loc + bp * M * 2;  // (x,y) per camera; broadcast loads
-        for (int c0 = lane * VEC; c0 < C; c0 += 32 * VEC) {
+        for (int c0 = lane; c0 < C; c0 += 32) {
             const int grp = c0 / gdim;
-            T acc = V::zero();
-            T gout = V::zero();
-            if (BACKWARD) gout = V::load(p.grad_out + bp * C + c0);
+            float acc = 0.f;
+            float gout = 0.f;
+            if (BACKWARD) gout = __ldg(p.grad_out + bp * C + c0);
             for (int m = 0; m < M; ++m) {
                 const float lx = __ldg(locp + 2 * m), ly = __ldg(locp + 2 * m + 1);
                 if (!(lx > 0.f && lx < 1.f && ly > 0.f && ly < 1.f)) continue;  // warp-uniform
@@ -115,72 +89,51 @@ __global__ void __launch_bounds__(kDafThreads) daf_kernel(const DafParams p) {
                 for (int l = 0; l < L; ++l) {
                     const Bilinear bl = bilinear_setup(lx, ly, lh[l], lw[l]);
                     const float *flev = fcam + static_cast<long long>(ls[l]) * C;
-                    T v[4];
+                    float v[4];
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) v[k] = bl.ok[k] ? V::load(flev + bl.row[k] * C) : V::zero();
+                    for (int k = 0; k < 4; ++k) v[k] = bl.ok[k] ? __ldg(flev + bl.row[k] * C) : 0.f;
                     const float wt = __ldg(p.weights + wbase + static_cast<long long>(l) * Gr);
                     if (!BACKWARD) {
-                        T val = V::zero();
+                        float val = 0.f;
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) V::fma(val, bl.w[k], v[k]);
-                        V::fma(acc, wt, val);
+                        for (int k = 0; k < 4; ++k) val = fmaf(bl.w[k], v[k], val);
+                        acc = fmaf(wt, val, acc);
                     } else {
                         // d(out)/d(feat corner) = bilinear weight * aggregation weight
                         float *gf = p.grad_feat + (fcam - p.feat) + static_cast<long long>(ls[l]) * C;
 #pragma unroll
                         for (int k = 0; k < 4; ++k)
-                            if (bl.ok[k]) V::atomic_add_scaled(gf + bl.row[k] * C, bl.w[k] * wt, gout);
+                            if (bl.ok[k]) atomicAdd(gf + bl.row[k] * C, (bl.w[k] * wt) * gout);
                         // d(out)/d(weight) = sampled value
-                        T val = V::zero();
+                        float val = 0.f;
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) V::fma(val, bl.w[k], v[k]);
-                        float gw = V::dot(gout, val);
+                        for (int k = 0; k < 4; ++k) val = fmaf(bl.w[k], v[k], val);
+                        const float gw = gout * val;
                         // d(out)/d(x_im), d(out)/d(y_im)   (cuda.cu:85-121)
-                        T dvx = V::zero(), dvy = V::zero();
-                        V::fma(dvx, -bl.hh, v[0]); V::fma(dvx, bl.hh, v[1]); V::fma(dvx, -bl.lh, v[2]); V::fma(dvx, bl.lh, v[3]);
-                        V::fma(dvy, -bl.hw, v[0]); V::fma(dvy, -bl.lw, v[1]); V::fma(dvy, bl.hw, v[2]); V::fma(dvy, bl.lw, v[3]);
-                        gx = fmaf(static_cast<float>(lw[l]) * wt, V::dot(gout, dvx), gx);
-                        gy = fmaf(static_cast<float>(lh[l]) * wt, V::dot(gout, dvy), gy);
-                        if (VEC == 4) {
-                            const int lanes_per_group = gdim / 4;
-#pragma unroll
-                            for (int o = 1; o < 32; o <<= 1)
-                                if (o < lanes_per_group) gw += __shfl_xor_sync(0xffffffffu, gw, o);
-                            if ((lane & (lanes_per_group - 1)) == 0) p.grad_weights[wbase + static_cast<long long>(l) * Gr] += gw;
-                        } else {
-                            atomicAdd(p.grad_weights + wbase + static_cast<long long>(l) * Gr, gw);
-                        }
+                        float dvx = 0.f, dvy = 0.f;
+                        dvx = fmaf(-bl.hh, v[0], dvx); dvx = fmaf(bl.hh, v[1], dvx); dvx = fmaf(-bl.lh, v[2], dvx); dvx = fmaf(bl.lh, v[3], dvx);
+                        dvy = fmaf(-bl.hw, v[0], dvy); dvy = fmaf(-bl.lw, v[1], dvy); dvy = fmaf(bl.hw, v[2], dvy); dvy = fmaf(bl.lw, v[3], dvy);
+                        gx = fmaf(static_cast<float>(lw[l]) * wt, gout * dvx, gx);
+                        gy = fmaf(static_cast<float>(lh[l]) * wt, gout * dvy, gy);
+                        atomicAdd(p.grad_weights + wbase + static_cast<long long>(l) * Gr, gw);
                     }
                 }
                 if (BACKWARD) {
                     float *gl = p.grad_loc + (bp * M + m) * 2;
-                    if (VEC == 4) {  // all 32 lanes are here (C % 128 == 0)
-#pragma unroll
-                        for (int o = 16; o > 0; o >>= 1) {
-                            gx += __shfl_xor_sync(0xffffffffu, gx, o);
-                            gy += __shfl_xor_sync(0xffffffffu, gy, o);
-                        }
-                        if (lane == 0) {
-                            // with several channel slices (C > 128) each slice adds its share in turn
-                            gl[0] += gx;
-                            gl[1] += gy;
-                        }
-                    } else {
-                        atomicAdd(gl, gx);
-                        atomicAdd(gl + 1, gy);
-                    }
+                    atomicAdd(gl, gx);
+                    atomicAdd(gl + 1, gy);
                 }
             }
-            if (!BACKWARD) V::store(p.out + bp * C + c0, acc);
+            if (!BACKWARD) p.out[bp * C + c0] = acc;
         }
     }
 }
 
 // ------------------------------------------------------------------------------------------------
 // Fast path (C % 128 == 0, a group = whole lanes, M*L <= 32): one warp per sampling point, and the
-// bilinear setup of each (camera, level) pair is computed by ONE lane instead of all 32 — the r01
-// profile showed the first-generation kernel to be instruction-bound (224 M warp instructions,
-// L2 at 27 %), almost all of it redundant warp-uniform setup arithmetic.
+// bilinear setup of each (camera, level) pair is computed by ONE lane instead of all 32 — a kernel
+// that repeats it in every lane is instruction-bound (224 M warp instructions, L2 at 27 %), almost
+// all of it redundant warp-uniform setup arithmetic.
 //   lane p < M*L      : pair p = (camera p / L, level p % L): gate, 4 corner rows (clamped to a valid
 //                       row), 4 corner weights (zero for corners outside the map) -> per-warp smem
 //   ballot of the gate: only visible pairs are visited, in ascending (camera, level) order
@@ -304,13 +257,41 @@ int launch_daf(const gf_daf_desc &d, const DafParams &dp, bool backward, int num
     const bool v4 = daf_vec4_ok(d);
     if (backward) {
         if (v4) daf_fast_kernel<true><<<grid, kDafThreads, 0, stream>>>(dp);
-        else daf_kernel<1, true><<<grid, kDafThreads, 0, stream>>>(dp);
+        else daf_kernel<true><<<grid, kDafThreads, 0, stream>>>(dp);
     } else {
         if (v4) daf_fast_kernel<false><<<grid, kDafThreads, 0, stream>>>(dp);
-        else daf_kernel<1, false><<<grid, kDafThreads, 0, stream>>>(dp);
+        else daf_kernel<false><<<grid, kDafThreads, 0, stream>>>(dp);
     }
     GF_CUDA_TRY(cudaGetLastError());
     return GF_OK;
+}
+
+// Random row gather: every warp sums rows of `row_floats` floats (a multiple of 128) picked by idx[] from a table -- the
+// access pattern of the sampling op without its arithmetic.  A warp reads 32 row numbers with one coalesced load and
+// keeps eight 512-byte row reads in flight (the op keeps four per visible pair).  With a table that fits L2 this
+// measures the L2 -> SM gather bandwidth the op can reach at most.
+__global__ void __launch_bounds__(256) gather_probe_kernel(const float *table, const int32_t *idx, long long n, int row_floats, float *sink) {
+    const int lane = threadIdx.x & 31;
+    const long long warp = (static_cast<long long>(blockIdx.x) * 256 + threadIdx.x) >> 5, warps = static_cast<long long>(gridDim.x) * 8;
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (long long i = warp * 32; i < n; i += warps * 32) {
+        const long long j = i + lane < n ? i + lane : n - 1;
+        const int mine = __ldg(idx + j);
+#pragma unroll 1
+        for (int k0 = 0; k0 < 32; k0 += 8) {
+            const float *row[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) row[k] = table + static_cast<long long>(__shfl_sync(0xffffffffu, mine, k0 + k)) * row_floats;
+            for (int c0 = lane * 4; c0 < row_floats; c0 += 128) {
+                float4 v[8];
+#pragma unroll
+                for (int k = 0; k < 8; ++k) v[k] = __ldg(reinterpret_cast<const float4 *>(row[k] + c0));   // eight loads in flight
+#pragma unroll
+                for (int k = 0; k < 8; ++k) { acc.x += v[k].x; acc.y += v[k].y; acc.z += v[k].z; acc.w += v[k].w; }
+            }
+        }
+    }
+    if (acc.x + acc.y + acc.z + acc.w == 123456.789f) sink[0] = acc.x;   // keeps the loads alive
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -439,3 +420,14 @@ int launch_daf_backward(const gf_daf_desc &d, const float *feat, const int32_t *
 }
 
 }  // namespace gf
+
+extern "C" int gf_debug_gather_probe(const float *table, const int32_t *idx, int64_t n, int32_t row_floats, float *sink,
+                                     gf_stream_t stream_) {
+    GF_REQUIRE(table && idx && sink && n > 0 && row_floats > 0 && row_floats % 128 == 0, GF_ERR_INVALID_ARG, "gather probe: bad argument");
+    int dev = 0, num_sms = 1;
+    GF_CUDA_TRY(cudaGetDevice(&dev));
+    GF_CUDA_TRY(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
+    gf::gather_probe_kernel<<<num_sms * 8, 256, 0, static_cast<cudaStream_t>(stream_)>>>(table, idx, n, row_floats, sink);
+    GF_CUDA_TRY(cudaGetLastError());
+    return GF_OK;
+}

@@ -92,13 +92,10 @@ __device__ __forceinline__ void walk_pairs_t(const BwdParams &p, GaussAcc<C, PRO
     }
 }
 
-#ifndef GF_BWD_WIDE
-#define GF_BWD_WIDE 1
-#endif
 template <int C, bool PROB>
 __device__ __forceinline__ void walk_pairs(const BwdParams &p, GaussAcc<C, PROB> &acc, BoxWalk &box, bool canon) {
     // wide rows need an even class count and a 16-byte aligned gradient tensor (uniform for the launch)
-    if (GF_BWD_WIDE && (C & 1) == 0 && (reinterpret_cast<uintptr_t>(p.gr.logits_grad) & 15) == 0)
+    if ((C & 1) == 0 && (reinterpret_cast<uintptr_t>(p.gr.logits_grad) & 15) == 0)
         walk_pairs_t<C, PROB, true>(p, acc, box, canon);
     else
         walk_pairs_t<C, PROB, false>(p, acc, box, canon);
@@ -326,22 +323,15 @@ static int launch_backward_t(const BwdParams &bp, const BwdWorkspace &ws, bool s
     GF_CUDA_TRY(cudaMemsetAsync(bp.canon, 0xFF, ws.cv_bytes, stream));
     const long long want = (static_cast<long long>(d.N) + 255) / 256;
     const int grid0 = static_cast<int>(want < 16ll * num_sms ? (want > 0 ? want : 1) : 16ll * num_sms);
-    auto launch_aux = [&](bool chained) -> int {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(grid0, B); cfg.blockDim = dim3(256); cfg.stream = stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr; cfg.numAttrs = (chained && pdl_enabled()) ? 1 : 0;
-        GF_CUDA_TRY(cudaLaunchKernelEx(&cfg, prob_aux_kernel, bp, static_cast<int>(C)));
-        return GF_OK;
-    };
     if (bp.bin_active) {
         // Canonical points (checked by the bin kernel itself): memset -> [prob_aux] -> pack -> list -> bin -> finish, and
         // the Gaussian-centric chain below finds the flag set and returns.  pack is launched in plain stream order (it
         // starts when everything above has completed); the kernels after it are chained to their predecessor.
         GF_CUDA_TRY(cudaMemsetAsync(ws.sums, 0, ws.sums_bytes, stream));   // accumulated with atomics
-        if (PROB) { int rc = launch_aux(false); if (rc != GF_OK) return rc; }
+        if (PROB) {
+            prob_aux_kernel<<<dim3(grid0, B), 256, 0, stream>>>(bp, C);
+            GF_CUDA_TRY(cudaGetLastError());
+        }
         SplatWorkspace fws;
         plan_forward_workspace(d, ws.fwd, &fws);
         int rc = launch_prep(d, bp.in, fws, 0u, stream, true);
@@ -353,7 +343,7 @@ static int launch_backward_t(const BwdParams &bp, const BwdWorkspace &ws, bool s
     } else {
         voxel_map_kernel<<<dim3(grid0, B), 256, 0, stream>>>(bp);   // plain stream order: never overlaps the previous call
         GF_CUDA_TRY(cudaGetLastError());
-        if (PROB) { int rc = launch_aux(true); if (rc != GF_OK) return rc; }
+        if (PROB) GF_CUDA_TRY(launch_chained(prob_aux_kernel, dim3(grid0, B), dim3(256), 0, stream, bp, C));
     }
     constexpr int kBwdThreads = bwd_threads(PROB);
     const int per_cta = kBwdThreads / 32;
@@ -393,21 +383,11 @@ int launch_backward(const gf_splat_desc &d, const gf_splat_inputs &in, const gf_
     bp.cv_block = ws.cv_block;
     bp.bin_active = backward_bin_eligible(bp.d, bp.in, bp.gr) ? 1 : 0;
     const bool prob = d.variant == GF_SPLAT_PROB;
-#define GF_CASE(CC)                                                                \
-    case CC:                                                                       \
-        return prob ? launch_backward_t<CC, true>(bp, ws, srt, num_sms, stream)    \
-                    : launch_backward_t<CC, false>(bp, ws, srt, num_sms, stream);
-    switch (d.C) {
-        GF_CASE(16)
-        GF_CASE(17)
-        GF_CASE(18)
-        GF_CASE(19)
-        GF_CASE(20)
-        default:
-            set_error("splat backward: class count C=%d is not compiled in (supported: 16..20)", d.C);
-            return GF_ERR_UNSUPPORTED;
-    }
-#undef GF_CASE
+    return dispatch_classes(d.C, "splat backward", [&](auto cc) {
+        constexpr int C = decltype(cc)::value;
+        return prob ? launch_backward_t<C, true>(bp, ws, srt, num_sms, stream)
+                    : launch_backward_t<C, false>(bp, ws, srt, num_sms, stream);
+    });
 }
 
 }  // namespace gf

@@ -10,8 +10,8 @@
 //     (cp.async.bulk.tensor.3d, boxes {8C, 4, 8} / {48, 4, 8} / {64, 4, 8} over [B*H][W][D*C]-shaped tensor maps;
 //     out-of-grid parts of a box are zero-filled by the hardware) -- every byte of the 46 MB gradient is read from
 //     global memory once, coalesced;
-//   * resolves the bin's ordered Gaussian list from the supertile list while the copies are in flight (Phase A of
-//     the render kernel);
+//   * resolves the bin's ordered Gaussian list from the supertile list while the copies are in flight (Phase A,
+//     resolve_bin_list in common.cuh, shared with the render kernel);
 //   * gives every listed Gaussian to EIGHT lanes (four Gaussians per warp at a time; warps take groups of four list
 //     entries from a shared counter): the lanes stride over the box clipped to the bin (92 voxels on average for the
 //     nuScenes workload -- a whole warp per Gaussian would spend more on its reduction than on the pairs), read their
@@ -21,10 +21,9 @@
 //   * bin_finish_kernel applies the per-Gaussian linear maps (finish(), splat_bwd_common.cuh) once per Gaussian.
 //
 // The accumulator is zero-filled by the host first.  Summation order across bins is not fixed (fp32 atomics), so two
-// runs may differ in the last bits; GF_B200_BWD=gauss selects the deterministic Gaussian-centric kernels, which also
-// serve every case this kernel does not cover (points not in canonical order, odd strides, misaligned tensors).
+// runs may differ in the last bits.  The Gaussian-centric kernels serve every case this kernel does not cover (points
+// not in canonical order, odd strides, misaligned tensors).
 #include <cuda.h>
-#include <cstdlib>
 
 #include "splat_bwd_common.cuh"
 
@@ -104,7 +103,7 @@ __device__ __forceinline__ int small_div(int i, int n) {
 template <int C, bool PROB>
 __global__ void __launch_bounds__(kBinThreads, 2) backward_bin_kernel(const BwdParams pb, const BinParams bp,
                                                                        const __grid_constant__ BinMaps maps) {
-    constexpr int NT = kBinThreads, NWARP = NT / 32, CP2 = (C + 1) / 2;
+    constexpr int NT = kBinThreads, CP2 = (C + 1) / 2;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     BinSmem<C, PROB> &sm = *reinterpret_cast<BinSmem<C, PROB> *>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -130,13 +129,11 @@ __global__ void __launch_bounds__(kBinThreads, 2) backward_bin_kernel(const BwdP
         if (PROB) tma_load_3d(&sm.aux[0], &maps.aux, binZ0 * 4, binY0, xr, &sm.bar);
     }
 
-    // ---- candidates: the ascending list of this bin's supertile (as walk_tile, splat_tile.cuh) ------------------
+    // ---- candidates: the ascending list of this bin's supertile ------------------------------------------------
     const int st_shift = 31 - __clz(bp.st);
     const int s = sample * bp.nsuper + (binX0 >> st_shift) * bp.nsy + (binY0 >> st_shift);
     const int ncand = bp.counts[s];
-    const int32_t *cand = bp.lists + static_cast<size_t>(s) * p.d.G;
     const PackedBox *boxes = bp.boxes + static_cast<size_t>(sample) * p.d.G;
-    const uint32_t bX1 = min(binX0 + kBinX, H) - 1, bY1 = min(binY0 + kBinY, W) - 1, bZ1 = min(binZ0 + kBinZ, D) - 1;
     bool tiles_ready = false;
 
     int cpos = 0;
@@ -145,51 +142,8 @@ __global__ void __launch_bounds__(kBinThreads, 2) backward_bin_kernel(const BwdP
         if (tid == 0) sm.next = 0;   // published by the barriers of Phase A
         if (tid <= kVolKeys) sm.hist[tid] = 0;
         // ======================= Phase A: ordered survivors of the box test ==========================
-        int nlist = 0;
-        while (cpos < ncand && nlist + NT <= kBinSeg) {
-            constexpr int kPre = 2;   // rounds fetched together (memory-level parallelism)
-            int gg[kPre];
-            uint4 bb[kPre];
-#pragma unroll
-            for (int u = 0; u < kPre; ++u) {
-                const int i = cpos + u * NT + tid;
-                gg[u] = i < ncand ? __ldg(cand + i) : -1;
-            }
-#pragma unroll
-            for (int u = 0; u < kPre; ++u)
-                bb[u] = gg[u] >= 0 ? __ldg(reinterpret_cast<const uint4 *>(boxes) + gg[u]) : make_uint4(1u, 1u, 1u, 1u);
-#pragma unroll
-            for (int u = 0; u < kPre; ++u) {
-                if (cpos >= ncand || nlist + NT > kBinSeg) break;   // uniform
-                const uint4 b = bb[u];
-                const uint32_t x0 = b.x & 0xffffu, x1 = b.x >> 16, y0 = b.y & 0xffffu, y1 = b.y >> 16,
-                               z0 = b.z & 0xffffu, z1 = b.z >> 16;
-                const bool hit = gg[u] >= 0 && x0 <= bX1 && x1 >= static_cast<uint32_t>(binX0) && y0 <= bY1 &&
-                                 y1 >= static_cast<uint32_t>(binY0) && z0 <= bZ1 && z1 >= static_cast<uint32_t>(binZ0) &&
-                                 b.w == 0u;
-                const int rx0 = max(static_cast<int>(x0) - binX0, 0), rx1 = min(static_cast<int>(x1) - binX0, kBinX - 1);
-                const int ry0 = max(static_cast<int>(y0) - binY0, 0), ry1 = min(static_cast<int>(y1) - binY0, kBinY - 1);
-                const int rz0 = max(static_cast<int>(z0) - binZ0, 0), rz1 = min(static_cast<int>(z1) - binZ0, kBinZ - 1);
-                const uint32_t xm = ((2u << rx1) - 1u) & ~((1u << rx0) - 1u);
-                const uint32_t ym = ((2u << ry1) - 1u) & ~((1u << ry0) - 1u);
-                const uint32_t zm = ((2u << rz1) - 1u) & ~((1u << rz0) - 1u);
-                const uint2 entry = make_uint2(xm | (ym << 8) | (zm << 16), static_cast<uint32_t>(gg[u]));
-                const uint32_t ballot = __ballot_sync(0xffffffffu, hit);
-                if (lane == 0) sm.warp_count[u & 1][warp] = __popc(ballot);
-                __syncthreads();
-                int off = nlist, total = 0;
-#pragma unroll
-                for (int k = 0; k < NWARP; ++k) {
-                    const int c = sm.warp_count[u & 1][k];
-                    if (k < warp) off += c;
-                    total += c;
-                }
-                if (hit) sm.list[off + __popc(ballot & lanemask_lt())] = entry;
-                nlist += total;
-                cpos += NT;
-            }
-            __syncthreads();
-        }
+        const int nlist = resolve_bin_list<NT, 2, kBinSeg>(p.d, bp.lists, s, ncand, cpos, boxes, binX0, binY0, binZ0, sm.list,
+                                                           sm.warp_count);
         // ---- order the entries by clipped-box volume (counting sort; the order of the sum does not matter here) ----
         int mykey[kBinSeg / NT];
 #pragma unroll
@@ -425,11 +379,7 @@ static bool make_map(CUtensorMap *m, const void *base, long long rows, int W, in
 
 // Can the bin-centric kernel serve this call (if the points turn out to be in canonical order on the device)?
 bool backward_bin_eligible(const gf_splat_desc &d, const gf_splat_inputs &in, const gf_splat_grads &gr) {
-    static const bool forced_off = [] {
-        const char *e = getenv("GF_B200_BWD");
-        return e && e[0] == 'g';   // GF_B200_BWD=gauss: the deterministic Gaussian-centric kernels
-    }();
-    if (forced_off || encode_tiled() == nullptr) return false;
+    if (encode_tiled() == nullptr) return false;
     if (static_cast<long long>(d.N) != static_cast<long long>(d.H) * d.W * d.D || d.N == 0 || d.G == 0) return false;
     if ((d.D & 3) != 0 || 8 * d.C > 256) return false;   // 16-byte strides of the tensor maps, box <= 256 elements
     auto al16 = [](const void *q) { return (reinterpret_cast<uintptr_t>(q) & 15u) == 0; };
@@ -446,17 +396,7 @@ static int launch_bin_t(const BwdParams &bp, const BinParams &np, const BinMaps 
     const size_t smem = sizeof(BinSmem<C, PROB>);
     // per call: the attribute is per device, and a process may drive several
     GF_CUDA_TRY(cudaFuncSetAttribute(backward_bin_kernel<C, PROB>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(nzc, nby, np.nbx * B);
-    cfg.blockDim = dim3(kBinThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
-    GF_CUDA_TRY(cudaLaunchKernelEx(&cfg, backward_bin_kernel<C, PROB>, bp, np, maps));
+    GF_CUDA_TRY(launch_chained(backward_bin_kernel<C, PROB>, dim3(nzc, nby, np.nbx * B), dim3(kBinThreads), smem, stream, bp, np, maps));
     const float *sums = np.sums;
     GF_CUDA_TRY(launch_chained(bin_finish_kernel<C, PROB>, dim3((d.G + 127) / 128, B), dim3(128), 0, stream, bp, sums));
     return GF_OK;
@@ -483,21 +423,10 @@ int launch_backward_bin(const BwdParams &bp, const SplatWorkspace &fws, float *s
     np.nsuper = fws.nsuper;
     np.nbx = (d.H + kBinX - 1) / kBinX;
     const bool prob = d.variant == GF_SPLAT_PROB;
-#define GF_CASE(CC)                                                      \
-    case CC:                                                             \
-        return prob ? launch_bin_t<CC, true>(bp, np, maps, stream)       \
-                    : launch_bin_t<CC, false>(bp, np, maps, stream);
-    switch (d.C) {
-        GF_CASE(16)
-        GF_CASE(17)
-        GF_CASE(18)
-        GF_CASE(19)
-        GF_CASE(20)
-        default:
-            set_error("splat backward: class count C=%d is not compiled in (supported: 16..20)", d.C);
-            return GF_ERR_UNSUPPORTED;
-    }
-#undef GF_CASE
+    return dispatch_classes(d.C, "splat backward", [&](auto cc) {
+        constexpr int C = decltype(cc)::value;
+        return prob ? launch_bin_t<C, true>(bp, np, maps, stream) : launch_bin_t<C, false>(bp, np, maps, stream);
+    });
 }
 
 }  // namespace gf

@@ -8,12 +8,8 @@ namespace gf {
 constexpr int kBigBox = 2048;
 // CTA shapes of the two pair kernels: the prob variant carries more per-thread state, so it trades resident
 // warps for registers (128 threads x 3 CTAs -> 168 registers) instead of spilling at 128.
-#ifndef GF_BWD_PROB_THREADS
-#define GF_BWD_PROB_THREADS 128
-#define GF_BWD_PROB_CTAS 3
-#endif
-constexpr int bwd_threads(bool prob) { return prob ? GF_BWD_PROB_THREADS : 256; }
-constexpr int bwd_ctas(bool prob) { return prob ? GF_BWD_PROB_CTAS : 2; }
+constexpr int bwd_threads(bool prob) { return prob ? 128 : 256; }
+constexpr int bwd_ctas(bool prob) { return prob ? 3 : 2; }
 
 struct BwdParams {
     gf_splat_desc d;

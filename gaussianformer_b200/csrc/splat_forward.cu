@@ -5,10 +5,6 @@
 //                       comment below); stray points are detected per voxel and re-evaluated exactly.
 // render_points_kernel  arbitrary points (N != H*W*D, several per voxel): one thread per point walks
 //                       the supertile list with the exact box test.
-// (Four tcgen05 formulations of the tile kernel were built and measured 1.9-2.1x slower than the SIMT kernel; they
-// were removed -- profiles/README.md "r02_a" and DESIGN.md section 4.2 keep the numbers and the reasons.)
-#include <cstdlib>
-
 #include "splat_tile.cuh"
 
 namespace gf {
@@ -25,7 +21,7 @@ extern thread_local cudaEvent_t g_ev_before, g_ev_after;  // measurement hooks (
 //     softmax cross-entropy partial sums of the CTA's voxels.
 // blockIdx = (z chunk, bin y, sample * nbx + bin x): one grid covers the whole batch.
 template <int C, bool PROB>
-__global__ void __launch_bounds__(kRenderThreads, PROB ? 3 : GF_RENDER_CTAS) render_tile_kernel(const RenderParams pb) {
+__global__ void __launch_bounds__(kRenderThreads, PROB ? 3 : 4) render_tile_kernel(const RenderParams pb) {
     constexpr int REC = rec_floats(C);
     constexpr int CP2 = (C + 1) / 2;   // packed class pairs
     constexpr int VOX = kVoxT;
@@ -399,9 +395,6 @@ static int launch_render_t(const RenderParams &rp, bool tile_path, int num_sms, 
     return GF_OK;
 }
 
-extern const int kSupportedClasses[] = {16, 17, 18, 19, 20};
-extern const int kNumSupportedClasses = 5;
-
 // render CTAs of the tile path per sample (= rows of out.ce_partials per sample)
 int render_ctas_per_sample(const gf_splat_desc &d) {
     return ((d.D + kBinZ - 1) / kBinZ) * ((d.W + kBinY - 1) / kBinY) * ((d.H + kBinX - 1) / kBinX);
@@ -432,21 +425,11 @@ int launch_render(const gf_splat_desc &d, const gf_splat_inputs &in, const gf_sp
     rp.vec_ok = (d.D & 3) == 0 && al16(in.pts) && al16(out.logits) && al16(out.logits_cn) && al16(out.bin_logits) &&
                 al16(out.density) && al16(out.probability) && (reinterpret_cast<uintptr_t>(out.argmax) & 3u) == 0;
     const bool prob = d.variant == GF_SPLAT_PROB;
-#define GF_CASE(CC)                                                                  \
-    case CC:                                                                         \
-        return prob ? launch_render_t<CC, true>(rp, tile_path, num_sms, stream)      \
-                    : launch_render_t<CC, false>(rp, tile_path, num_sms, stream);
-    switch (d.C) {
-        GF_CASE(16)
-        GF_CASE(17)
-        GF_CASE(18)
-        GF_CASE(19)
-        GF_CASE(20)
-        default:
-            set_error("splat: class count C=%d is not compiled in (supported: 16..20)", d.C);
-            return GF_ERR_UNSUPPORTED;
-    }
-#undef GF_CASE
+    return dispatch_classes(d.C, "splat", [&](auto cc) {
+        constexpr int C = decltype(cc)::value;
+        return prob ? launch_render_t<C, true>(rp, tile_path, num_sms, stream)
+                    : launch_render_t<C, false>(rp, tile_path, num_sms, stream);
+    });
 }
 
 }  // namespace gf

@@ -11,8 +11,6 @@
 //                      integer box, and one ballot bit per supertile (16x16 columns) it overlaps.
 //   list_kernel        one CTA per supertile: popcount-scan of the mask words -> ascending
 //                      Gaussian index list (ascending order == the reference's stable sort order).
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace gf {
@@ -236,14 +234,8 @@ __global__ void __launch_bounds__(kListThreads) list_kernel(const ListParams p) 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 int plan_forward_workspace(const gf_splat_desc &d, void *base, SplatWorkspace *ws) {
-    // supertile edge in columns: a multiple of both render bin edges (8 and 4); GF_B200_ST overrides
-    static int st_default = 0;
-    if (st_default == 0) {
-        const char *e = getenv("GF_B200_ST");
-        const int v = e ? atoi(e) : 16;
-        st_default = (v >= 8 && (v & (v - 1)) == 0) ? v : 16;
-    }
-    int st = st_default;
+    // supertile edge in columns: a power of two and a multiple of both render bin edges (8 and 4)
+    int st = 16;
     const size_t budget = size_t(512) << 20;
     while (true) {
         const size_t ns = size_t((d.H + st - 1) / st) * size_t((d.W + st - 1) / st);

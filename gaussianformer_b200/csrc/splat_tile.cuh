@@ -1,25 +1,17 @@
 // The tile walker of the render kernel: a CTA owns a bin of 8 x 4 columns x 16 z; it resolves its own ordered
 // Gaussian list from the supertile list (Phase A), streams the records through a shared-memory ring (Phase B)
 // and lets every lane walk ITS OWN hits of a batch in ascending Gaussian order (lane-private traversal).
-//
-// Measured and removed (profiles/README.md has the numbers): warp-uniform traversal (first generation), a warp =
-// the bin's 8 x 4 columns at one z quad, 64-record batches, the software-pipelined and the branch-free fused step,
-// 2 voxels per thread, 3 CTAs per SM, a K split of the last-round bins, early candidate prefetch.
 #pragma once
 #include "splat_render.cuh"
 
 namespace gf {
 
-#ifndef GF_RENDER_CTAS
-#define GF_RENDER_CTAS 4   // resident CTAs per SM the base tile kernel is compiled for
-#endif
 constexpr int kVoxT = 4;        // voxels per thread: a z quad
 constexpr int kQuadSeg = 512;   // list entries resolved per segment
 constexpr int kBatch = 32;      // records staged per ring slot; a lane keeps its hit mask of a batch in one word
-#ifndef GF_TILE_RING
-#define GF_TILE_RING 5   // measured: 5, 6, 7 slots 72.0 us per step, 4 and 8 slots 73.4 us
-#endif
-constexpr int kRing = GF_TILE_RING;   // ring slots: a warp may run up to kRing-2 batches ahead of the slowest one
+// ring slots: a warp may run up to kRing-2 batches ahead of the slowest one
+// (measured on a B200 before the H100 port: 5, 6, 7 slots 72.0 us per step, 4 and 8 slots 73.4 us)
+constexpr int kRing = 5;
 
 // Shared-memory row of a staged record: the 128-byte record followed by 16 bytes of padding, so that chunk c of row j
 // starts at bank group (j + c) mod 8 and lanes of one warp reading the same chunk of DIFFERENT records fall into
@@ -83,7 +75,6 @@ __device__ __forceinline__ void walk_tile(const RenderParams &p, RenderSmem<C> &
     constexpr int NT = kRenderThreads, NWARP = NT / 32, VOX = kVoxT;
     constexpr uint32_t VMASK = (1u << VOX) - 1u;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int H = p.d.H, W = p.d.W, D = p.d.D;
     if (tid == 0) {
 #pragma unroll
         for (int r = 0; r < kRing; ++r) {
@@ -99,8 +90,6 @@ __device__ __forceinline__ void walk_tile(const RenderParams &p, RenderSmem<C> &
     const int st_shift = 31 - __clz(p.st);
     const int s = (binX0 >> st_shift) * p.nsy + (binY0 >> st_shift);
     const int ncand = p.counts[s];
-    const int32_t *cand = p.lists + static_cast<size_t>(s) * p.d.G;
-    const uint32_t bX1 = min(binX0 + kBinX, H) - 1, bY1 = min(binY0 + kBinY, W) - 1, bZ1 = min(binZ0 + kBinZ, D) - 1;
 
     int cpos = 0;
     while (cpos < ncand) {
@@ -109,51 +98,8 @@ __device__ __forceinline__ void walk_tile(const RenderParams &p, RenderSmem<C> &
         const long long tA0 = clock64();
 #endif
         // ======================= Phase A: ordered survivors of the box test ==========================
-        int nlist = 0;
-        while (cpos < ncand && nlist + NT <= kQuadSeg) {
-            constexpr int kPre = 4;   // rounds fetched together (memory-level parallelism)
-            int gg[kPre];
-            uint4 bb[kPre];
-#pragma unroll
-            for (int u = 0; u < kPre; ++u) {
-                const int i = cpos + u * NT + tid;
-                gg[u] = i < ncand ? __ldg(cand + i) : -1;
-            }
-#pragma unroll
-            for (int u = 0; u < kPre; ++u)
-                bb[u] = gg[u] >= 0 ? __ldg(reinterpret_cast<const uint4 *>(p.boxes) + gg[u]) : make_uint4(1u, 1u, 1u, 1u);
-#pragma unroll
-            for (int u = 0; u < kPre; ++u) {
-                if (cpos >= ncand || nlist + NT > kQuadSeg) break;   // uniform
-                const uint4 b = bb[u];
-                const uint32_t x0 = b.x & 0xffffu, x1 = b.x >> 16, y0 = b.y & 0xffffu, y1 = b.y >> 16,
-                               z0 = b.z & 0xffffu, z1 = b.z >> 16;
-                const bool hit = gg[u] >= 0 && x0 <= bX1 && x1 >= static_cast<uint32_t>(binX0) && y0 <= bY1 &&
-                                 y1 >= static_cast<uint32_t>(binY0) && z0 <= bZ1 && z1 >= static_cast<uint32_t>(binZ0) &&
-                                 b.w == 0u;
-                const int rx0 = max(static_cast<int>(x0) - binX0, 0), rx1 = min(static_cast<int>(x1) - binX0, kBinX - 1);
-                const int ry0 = max(static_cast<int>(y0) - binY0, 0), ry1 = min(static_cast<int>(y1) - binY0, kBinY - 1);
-                const int rz0 = max(static_cast<int>(z0) - binZ0, 0), rz1 = min(static_cast<int>(z1) - binZ0, kBinZ - 1);
-                const uint32_t xm = ((2u << rx1) - 1u) & ~((1u << rx0) - 1u);
-                const uint32_t ym = ((2u << ry1) - 1u) & ~((1u << ry0) - 1u);
-                const uint32_t zm = ((2u << rz1) - 1u) & ~((1u << rz0) - 1u);
-                const uint2 entry = make_uint2(xm | (ym << 8) | (zm << 16), static_cast<uint32_t>(gg[u]));
-                const uint32_t ballot = __ballot_sync(0xffffffffu, hit);
-                if (lane == 0) sm.warp_count[u & 1][warp] = __popc(ballot);
-                __syncthreads();
-                int off = nlist, total = 0;
-#pragma unroll
-                for (int k = 0; k < NT / 32; ++k) {
-                    const int c = sm.warp_count[u & 1][k];
-                    if (k < warp) off += c;
-                    total += c;
-                }
-                if (hit) sm.list[off + __popc(ballot & lanemask_lt())] = entry;
-                nlist += total;
-                cpos += NT;
-            }
-            __syncthreads();
-        }
+        const int nlist = resolve_bin_list<NT, 4, kQuadSeg>(p.d, p.lists, s, ncand, cpos, p.boxes, binX0, binY0, binZ0, sm.list,
+                                                            sm.warp_count);
         // pad the last batch with empty entries (all-zero masks, so nobody visits them)
         if (tid < kBatch && nlist + tid < ((nlist + kBatch - 1) / kBatch) * kBatch) sm.list[nlist + tid] = make_uint2(0u, 0u);
         __syncthreads();

@@ -20,18 +20,9 @@ int gf_debug_set_render_events(void *before, void *after);
 /* Random row gather over a table (row i = row_floats floats, a multiple of 128; idx[n] int32 row numbers, device):
  * the access pattern of the sampling op without its arithmetic.  With an L2-resident table the achieved
  * n * row_floats * 4 bytes / time is the L2 -> SM gather bandwidth that bounds gf_daf_forward on uncorrelated
- * sampling points (bench.py: `daf_roof`). */
+ * sampling points (tools/daf_experiments.py). */
 int gf_debug_gather_probe(const float *table, const int32_t *idx, int64_t n, int32_t row_floats, float *sink,
                           gf_stream_t stream);
-
-/* EXPERIMENT (measured, not the product path): gf_daf_forward with the 2 x 2 x C corner block of every visible
- * (camera, level) pair fetched as one cp.async.bulk.tensor box {C, 2, 2, 1} from per-level tensor maps
- * [B*M][h_l][w_l][C]; hardware out-of-bounds zero fill replaces the corner validity tests
- * (deformable_aggregation_cuda.cu:31-49).  host_shape [L,2] / host_start [L] are HOST copies of spatial_shape /
- * scale_start_index (the tensor maps are encoded on the host).  C in {128, 256}. */
-int gf_debug_daf_forward_tma(const gf_daf_desc *desc, const float *mc_ms_feat, const int32_t *host_shape,
-                             const int32_t *host_start, const float *sample_location, const float *weights,
-                             float *output, gf_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -89,9 +89,9 @@ def assert_grad_parity(mine, ref64, ref32, what="", k=K_FLOOR, extra_floor=0.0):
     """Gradient parity gate.  BASELINE.md states ``|new - ref| <= 1e-5 + 1e-4*|ref|`` for gradients too; an entry
     is a sum of 10^2..10^6 signed fp32 terms, so where that cannot hold the bound is the MEASURED fp32 floor of the
     reference arithmetic on the same tensor: ``k * max|fp32 oracle - fp64 oracle|`` (``extra_floor``: the same
-    figure for a reference-op golden, when one is compared).  Measured at the BASELINE sizes
-    (profiles/r02_parity/*.json): cfg 2 and 3 hold the elementwise gate on every entry; the prob configs leave
-    <= 60 of 10^5 entries to the floor rule, with the new op 1-20x CLOSER to the fp64 oracle than the reference op."""
+    figure for a reference-op golden, when one is compared).  Measured at the BASELINE sizes: cfg 2 and 3 hold the
+    elementwise gate on every entry; the prob configs leave <= 60 of 10^5 entries to the floor rule, with the new op
+    1-20x CLOSER to the fp64 oracle than the reference op."""
     mine = np.asarray(mine, np.float64)
     ref64 = np.asarray(ref64, np.float64)
     err = np.abs(mine - ref64)

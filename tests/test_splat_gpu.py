@@ -341,7 +341,7 @@ def test_miou_is_unchanged():
     decided voxels; over ALL voxels (numerical ties included) within 1e-4 + K x the measured distance between the
     oracle's own fp32 and fp64 builds (the fp32 floor of the arithmetic on this sample, printed).
     The full-size op-vs-op version of this test is tests/test_parity_full_gpu.py (0 differences against the reference
-    op on configs 2, 3 and 4, profiles/r02_parity/)."""
+    op on configs 2, 3 and 4)."""
     from gaussianformer_b200.metric import miou_parity, synthetic_labels
     kw, inp, variant = h.splat_case("gs144000", 5, False, dict(G=20000))
     m = h.make_module(kw, variant)

@@ -1,6 +1,6 @@
 """Builds an alternative libgf_b200 with extra nvcc flags for A/B measurements:
-    python tools/build_variant.py ring0 -DGF_BWD_RING=0
-writes gaussianformer_b200/csrc/variants/libgf_b200_ring0.so; select it with GF_B200_LIB=<path>."""
+    python tools/build_variant.py timing -DGF_RENDER_TIMING
+writes gaussianformer_b200/csrc/variants/libgf_b200_timing.so; select it with GF_B200_LIB=<path>."""
 import os, subprocess, sys
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, ROOT)

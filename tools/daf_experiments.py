@@ -1,13 +1,11 @@
-"""Sampling-op experiments on one GPU: the L2 -> SM gather roof (random 512-byte rows of the 88 MB feature table), the
-product kernel against it on the uncorrelated and on the projected (correlated) workload, and the TMA corner-box
-variant (gf_debug_daf_forward_tma).  Prints one JSON object."""
+"""Sampling-op experiments on one GPU: the L2 -> SM gather roof (random 512-byte rows of the 88 MB feature table) and the
+product kernel against it on the uncorrelated and on the projected (correlated) workload.  Prints one JSON object."""
 import ctypes, json, os, sys
 import torch
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, ROOT)
 from gaussianformer_b200 import _lib  # noqa: E402
 from gaussianformer_b200.ops import DeformableAggregationFunction as DAF  # noqa: E402
-from gaussianformer_b200.ops.deformable_aggregation import _desc  # noqa: E402
 from gaussianformer_b200.synthetic import make_daf_inputs, make_daf_inputs_projected  # noqa: E402
 
 dev = torch.device("cuda")
@@ -68,20 +66,10 @@ def run_case(tag, fms, loc, w):
     ms_same = timeit(lambda: _lib.check(L_.gf_debug_gather_probe(ctypes.c_void_p(feat.data_ptr()), ctypes.c_void_p(idx_same.data_ptr()),
                                                                   idx_same.numel(), 128, ctypes.c_void_p(sink2.data_ptr()), stream())))
     ms = timeit(lambda: DAF.apply(feat, shape, start, loc, w))
-    ref = DAF.apply(feat, shape, start, loc, w)
-    d = _desc(feat, shape, loc, w)
-    hs = (ctypes.c_int32 * (2 * shape.shape[0]))(*[int(v) for v in shape.cpu().flatten().tolist()])
-    hst = (ctypes.c_int32 * shape.shape[0])(*[int(v) for v in start.cpu().tolist()])
-    o2 = torch.empty_like(ref)
-    call = lambda: _lib.check(L_.gf_debug_daf_forward_tma(ctypes.byref(d), ctypes.c_void_p(feat.data_ptr()), hs, hst, ctypes.c_void_p(loc.data_ptr()),
-                                                          ctypes.c_void_p(w.data_ptr()), ctypes.c_void_p(o2.data_ptr()), stream()))
-    ms_tma = timeit(call)
-    err = float((o2 - ref).abs().max())
     out[tag] = {"visible_pairs": pairs, "visible_fraction": float(vis.float().mean()), "gather_bytes": gathered,
                 "fwd_ms": ms, "gather_gbs": gathered / (ms * 1e-3) / 1e9, "frac_of_uniform_88MB_probe": gathered / (ms * 1e-3) / 1e9 / roof,
                 "same_rows_probe_ms": ms_same, "same_rows_probe_gbs": idx_same.numel() * 512 / (ms_same * 1e-3) / 1e9,
-                "frac_of_same_rows_probe": ms_same / ms,
-                "tma_fwd_ms": ms_tma, "tma_max_abs_diff_vs_product": err}
+                "frac_of_same_rows_probe": ms_same / ms}
 
 
 run_case("uncorrelated", fms, loc, w)

@@ -3,16 +3,11 @@
 # synccheck and initcheck on the same selection.  Usage (through gpurun): bash tools/sanitize.sh [tools...]
 set +e
 out=gpurun_out/sanitize; mkdir -p $out
-sel='goldens and not mid or other_class_counts or in_kernel or fused_epilogue or misaligned or status_codes or zero_points or generic_points or unaligned or daf_forward_backward or daf_matches or feature_maps or fused_forward or tma or batched_launch or shared_points'
+sel='goldens and not mid or other_class_counts or in_kernel or fused_epilogue or misaligned or status_codes or zero_points or generic_points or unaligned or daf_forward_backward or daf_matches or feature_maps or fused_forward or batched_launch or shared_points'
 tools=${@:-memcheck racecheck synccheck initcheck}
 for tool in $tools; do
-  extra=""
-  ksel="$sel"
-  # synccheck tracks a bounded number of mbarriers: the debug-only TMA sampling variant (a ring of four per warp, tens of
-  # thousands of warps) overflows it, and a larger table starves the tool of memory -- leave that one test out here
-  if [ $tool = synccheck ]; then ksel="($sel) and not corner_box"; fi
-  timeout 1500 compute-sanitizer --tool $tool $extra --error-exitcode 7 --print-limit 30 --log-file $out/$tool.log \
-      python -m pytest tests/test_splat_gpu.py tests/test_cabi_gpu.py tests/test_batch_fused_gpu.py tests/test_daf_gpu.py -m gpu -q -x -k "$ksel" > $out/$tool.pytest.log 2>&1
+  timeout 1500 compute-sanitizer --tool $tool --error-exitcode 7 --print-limit 30 --log-file $out/$tool.log \
+      python -m pytest tests/test_splat_gpu.py tests/test_cabi_gpu.py tests/test_batch_fused_gpu.py tests/test_daf_gpu.py -m gpu -q -x -k "$sel" > $out/$tool.pytest.log 2>&1
   echo "$tool rc=$? : $(tail -1 $out/$tool.pytest.log)"
   grep -E "ERROR SUMMARY|RACECHECK SUMMARY" $out/$tool.log | tail -2
   grep -E "^=========     at|Invalid|Uninitialized|hazard|Barrier error" $out/$tool.log | sort | uniq -c | sort -rn | head -12

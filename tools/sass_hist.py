@@ -1,5 +1,5 @@
 """Static SASS opcode histograms of the main kernels (cuobjdump -sass of the in-tree library; modifiers stripped).
-    python tools/sass_hist.py > profiles/r02_sass_opcode_histograms.txt"""
+    python tools/sass_hist.py"""
 import collections, os, re, subprocess, sys
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 LIB = os.path.join(ROOT, "gaussianformer_b200", "csrc", "libgf_b200.so")
@@ -8,7 +8,7 @@ KERNELS = [("render_tile_kernel<18,false>", "_ZN2gf18render_tile_kernelILi18ELb0
            ("backward_bin_kernel<18,false>", "backward_bin_kernelILi18ELb0"),
            ("backward_bin_kernel<18,true>", "backward_bin_kernelILi18ELb1"),
            ("pack_mask_kernel", "pack_mask_kernel"), ("list_kernel", "list_kernel"),
-           ("daf_fast_kernel<fwd>", "daf_fast_kernelILb0"), ("daf_tma_kernel (experiment)", "daf_tma_kernel")]
+           ("daf_fast_kernel<fwd>", "daf_fast_kernelILb0")]
 sass = subprocess.run(["cuobjdump", "-sass", LIB], capture_output=True, text=True).stdout
 funcs, cur = {}, None
 for line in sass.splitlines():
@@ -22,8 +22,7 @@ for line in sass.splitlines():
             funcs[cur].append(body.split()[0].split(".")[0].rstrip(";"))
 print("SASS opcode histograms (static instruction counts per kernel, cuobjdump -sass of the in-tree library; modifiers stripped).")
 print("What to look for: render = LDGSTS (cp.async ring) + SYNCS (mbarrier) + FFMA2 + MUFU, no tensor / TMA opcodes (SIMT by measurement, DESIGN.md 4.1);")
-print("backward_bin = UTMALDG (cp.async.bulk.tensor.3d tile copies) + SYNCS + REDG/ATOMG (raw-sum accumulation) + SHFL (8-lane transposing reduction);")
-print("daf_tma (experiment) = UTMALDG (4-D corner boxes).\n")
+print("backward_bin = UTMALDG (cp.async.bulk.tensor.3d tile copies) + SYNCS + REDG/ATOMG (raw-sum accumulation) + SHFL (8-lane transposing reduction).\n")
 for name, key in KERNELS:
     hit = [f for f in funcs if key in f]
     if not hit:

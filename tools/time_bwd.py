@@ -1,4 +1,4 @@
-"""C-ABI backward timing: python tools/time_bwd.py [config] [batch]   (GF_B200_BWD=gauss selects the Gaussian-centric kernels)"""
+"""C-ABI backward timing: python tools/time_bwd.py [config] [batch]"""
 import os, sys
 import torch
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
@@ -32,4 +32,4 @@ for _ in range(10):
     run()
 b.record()
 torch.cuda.synchronize()
-print(f"{cfg} B={B} bwd={os.environ.get('GF_B200_BWD', 'bin')}: {a.elapsed_time(b) / 10:.4f} ms per call, {a.elapsed_time(b) / 10 / B:.4f} ms per sample; |g_means| {float(out[0].abs().sum()):.6e}")
+print(f"{cfg} B={B}: {a.elapsed_time(b) / 10:.4f} ms per call, {a.elapsed_time(b) / 10 / B:.4f} ms per sample; |g_means| {float(out[0].abs().sum()):.6e}")
