@@ -5,6 +5,7 @@
 #include <cstring>
 
 #include "common.cuh"
+#include "daf_pair.cuh"
 #include "gf_b200_debug.h"
 
 namespace gf {
@@ -35,22 +36,10 @@ int launch_backward(const gf_splat_desc &d, const gf_splat_inputs &in, const gf_
 int render_ctas_per_sample(const gf_splat_desc &d);
 extern thread_local cudaEvent_t g_ev_before, g_ev_after;
 
-struct DafParams;
-int launch_daf_forward(const gf_daf_desc &d, const float *feat, const int32_t *shape, const int32_t *start,
-                       const float *loc, const float *weights, float *out, int num_sms, cudaStream_t stream);
+int launch_daf(const DafParams &p, bool backward, int num_sms, cudaStream_t stream);
 int launch_daf_format(const gf_daf_format_desc &d, float *const *maps, float *table, bool inverse, cudaStream_t stream);
-int launch_daf_backward(const gf_daf_desc &d, const float *feat, const int32_t *shape, const int32_t *start,
-                        const float *loc, const float *weights, const float *grad_out, float *grad_feat,
-                        float *grad_loc, float *grad_weights, int num_sms, cudaStream_t stream);
-
 bool daf_fused_supported(const gf_daf_desc &d, int K);
-int launch_daf_fused_forward(const gf_daf_desc &d, int K, const float *feat, const int32_t *shape, const int32_t *start,
-                             const float *loc, const float *logits, const uint8_t *pmask, const uint8_t *wmask,
-                             float *out, float *stats, int num_sms, cudaStream_t stream);
-int launch_daf_fused_backward(const gf_daf_desc &d, int K, const float *feat, const int32_t *shape, const int32_t *start,
-                              const float *loc, const float *logits, const uint8_t *pmask, const uint8_t *wmask,
-                              const float *stats, const float *out, const float *grad_out, float *grad_feat,
-                              float *grad_loc, float *grad_logits, int num_sms, cudaStream_t stream);
+int launch_daf_fused(const DafFusedParams &p, bool backward, int num_sms, cudaStream_t stream);
 
 thread_local cudaEvent_t g_ev_before = nullptr, g_ev_after = nullptr;
 
@@ -239,8 +228,9 @@ int gf_daf_forward(const gf_daf_desc *desc, const float *feat, const int32_t *sh
     int num_sms = 1;
     rc = num_sms_of_current_device(&num_sms);
     if (rc != GF_OK) return rc;
-    return launch_daf_forward(*desc, feat, shape, start, loc, weights, output, num_sms,
-                              static_cast<cudaStream_t>(stream_));
+    DafParams p{};
+    p.d = *desc; p.feat = feat; p.shape = shape; p.start = start; p.loc = loc; p.weights = weights; p.out = output;
+    return launch_daf(p, false, num_sms, static_cast<cudaStream_t>(stream_));
 }
 
 int gf_daf_backward(const gf_daf_desc *desc, const float *feat, const int32_t *shape, const int32_t *start,
@@ -256,8 +246,10 @@ int gf_daf_backward(const gf_daf_desc *desc, const float *feat, const int32_t *s
     int num_sms = 1;
     rc = num_sms_of_current_device(&num_sms);
     if (rc != GF_OK) return rc;
-    return launch_daf_backward(*desc, feat, shape, start, loc, weights, grad_output, grad_feat, grad_loc,
-                               grad_weights, num_sms, static_cast<cudaStream_t>(stream_));
+    DafParams p{};
+    p.d = *desc; p.feat = feat; p.shape = shape; p.start = start; p.loc = loc; p.weights = weights;
+    p.grad_out = grad_output; p.grad_feat = grad_feat; p.grad_loc = grad_loc; p.grad_weights = grad_weights;
+    return launch_daf(p, true, num_sms, static_cast<cudaStream_t>(stream_));
 }
 
 static int check_daf_fused(const gf_daf_fused_desc *fd) {
@@ -291,8 +283,10 @@ int gf_daf_fused_forward(const gf_daf_fused_desc *fd, const float *feat, const i
     int num_sms = 1;
     rc = num_sms_of_current_device(&num_sms);
     if (rc != GF_OK) return rc;
-    return launch_daf_fused_forward(fd->d, fd->pts_per_anchor, feat, shape, start, loc, logits, point_mask, weight_mask,
-                                    output, stats, num_sms, static_cast<cudaStream_t>(stream_));
+    DafFusedParams p{};
+    p.d = fd->d; p.K = fd->pts_per_anchor; p.feat = feat; p.shape = shape; p.start = start; p.loc = loc; p.logits = logits;
+    p.pmask = point_mask; p.wmask = weight_mask; p.out = output; p.stats = stats;
+    return launch_daf_fused(p, false, num_sms, static_cast<cudaStream_t>(stream_));
 }
 
 int gf_daf_fused_backward(const gf_daf_fused_desc *fd, const float *feat, const int32_t *shape, const int32_t *start,
@@ -310,9 +304,11 @@ int gf_daf_fused_backward(const gf_daf_fused_desc *fd, const float *feat, const 
     int num_sms = 1;
     rc = num_sms_of_current_device(&num_sms);
     if (rc != GF_OK) return rc;
-    return launch_daf_fused_backward(fd->d, fd->pts_per_anchor, feat, shape, start, loc, logits, point_mask, weight_mask,
-                                     stats, output, grad_output, grad_feat, grad_loc, grad_logits, num_sms,
-                                     static_cast<cudaStream_t>(stream_));
+    DafFusedParams p{};
+    p.d = fd->d; p.K = fd->pts_per_anchor; p.feat = feat; p.shape = shape; p.start = start; p.loc = loc; p.logits = logits;
+    p.pmask = point_mask; p.wmask = weight_mask; p.stats = const_cast<float *>(stats); p.out_saved = output;
+    p.grad_out = grad_output; p.grad_feat = grad_feat; p.grad_loc = grad_loc; p.grad_logits = grad_logits;
+    return launch_daf_fused(p, true, num_sms, static_cast<cudaStream_t>(stream_));
 }
 
 int gf_daf_format(const gf_daf_format_desc *desc, float *const *maps, float *table, int inverse, gf_stream_t stream_) {

@@ -7,25 +7,12 @@
 //   * lanes span the channel vector in float4 slices, so each of the 4 bilinear corners is one
 //     coalesced 16-byte-per-lane read of a 512-byte feature row (channels-last layout);
 //   * the camera gate and all bilinear coefficients are warp-uniform;
-//   * backward: feature gradients go out as 16-byte vector atomics (one per lane per corner),
-//     weight gradients are reduced over the lanes of a group with shuffles and written by one
-//     lane, location gradients are reduced over the warp — no scalar atomic storms.
+//   * backward: vector atomics for the feature gradients and shuffle reductions for the weight and
+//     location gradients (visit_pairs, daf_pair.cuh) — no scalar atomic storms.
 #include "daf_pair.cuh"
 #include "gf_b200_debug.h"
 
 namespace gf {
-
-struct DafParams {
-    gf_daf_desc d;
-    const float *feat;
-    const int32_t *shape;
-    const int32_t *start;
-    const float *loc;
-    const float *weights;
-    float *out;               // forward
-    const float *grad_out;    // backward
-    float *grad_feat, *grad_loc, *grad_weights;
-};
 
 struct Bilinear {
     float w[4];          // corner weights (tl, tr, bl, br)
@@ -62,14 +49,8 @@ __global__ void __launch_bounds__(kDafThreads) daf_kernel(const DafParams p) {
     const int gdim = C / Gr;
     const long long npts = static_cast<long long>(p.d.batch) * p.d.num_pts;
     const long long warps = static_cast<long long>(gridDim.x) * (kDafThreads / 32);
-    // level table in shared memory (dynamically indexed registers would spill to local memory)
     __shared__ int lh[kMaxLevels], lw[kMaxLevels], ls[kMaxLevels];
-    if (threadIdx.x < L) {
-        lh[threadIdx.x] = p.shape[2 * threadIdx.x];
-        lw[threadIdx.x] = p.shape[2 * threadIdx.x + 1];
-        ls[threadIdx.x] = p.start[threadIdx.x];
-    }
-    __syncthreads();
+    load_level_table(p.d, p.shape, p.start, lh, lw, ls);
 
     for (long long bp = static_cast<long long>(blockIdx.x) * (kDafThreads / 32) + (threadIdx.x >> 5); bp < npts; bp += warps) {
         const int b = static_cast<int>(bp / p.d.num_pts);
@@ -133,27 +114,18 @@ __global__ void __launch_bounds__(kDafThreads) daf_kernel(const DafParams p) {
 // Fast path (C % 128 == 0, a group = whole lanes, M*L <= 32): one warp per sampling point, and the
 // bilinear setup of each (camera, level) pair is computed by ONE lane instead of all 32 — a kernel
 // that repeats it in every lane is instruction-bound (224 M warp instructions, L2 at 27 %), almost
-// all of it redundant warp-uniform setup arithmetic.
-//   lane p < M*L      : pair p = (camera p / L, level p % L): gate, 4 corner rows (clamped to a valid
-//                       row), 4 corner weights (zero for corners outside the map) -> per-warp smem
-//   ballot of the gate: only visible pairs are visited, in ascending (camera, level) order
-//   every visit       : 2-3 uniform LDS.128 for the setup, one weight load, 4 coalesced 16-byte row
-//                       loads per lane, 16 FMAs
+// all of it redundant warp-uniform setup arithmetic.  The setup and the visit are setup_pairs and
+// visit_pairs (daf_pair.cuh).
 // ------------------------------------------------------------------------------------------------
 template <bool BACKWARD>
 __global__ void __launch_bounds__(kDafThreads, BACKWARD ? 3 : 4) daf_fast_kernel(const DafParams p) {
     __shared__ int lh[kMaxLevels], lw[kMaxLevels], ls[kMaxLevels];
     __shared__ __align__(16) PairSetup s_pair[kDafThreads / 32][32];
-    if (threadIdx.x < p.d.num_scale) {
-        lh[threadIdx.x] = p.shape[2 * threadIdx.x];
-        lw[threadIdx.x] = p.shape[2 * threadIdx.x + 1];
-        ls[threadIdx.x] = p.start[threadIdx.x];
-    }
-    __syncthreads();
+    load_level_table(p.d, p.shape, p.start, lh, lw, ls);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int C = p.d.num_embeds, M = p.d.num_cams, L = p.d.num_scale, Gr = p.d.num_groups, F = p.d.num_feat;
     const int npair = M * L;
-    const int gdim = C / Gr;
+    const int gdim = C / Gr, lanes_per_group = gdim / 4;
     const long long npts = static_cast<long long>(p.d.batch) * p.d.num_pts;
     const long long warps = static_cast<long long>(gridDim.x) * (kDafThreads / 32);
     PairSetup *mine = s_pair[warp];
@@ -162,105 +134,35 @@ __global__ void __launch_bounds__(kDafThreads, BACKWARD ? 3 : 4) daf_fast_kernel
 
     for (long long bp = static_cast<long long>(blockIdx.x) * (kDafThreads / 32) + warp; bp < npts; bp += warps) {
         const int b = small_index ? static_cast<int>(bp) / p.d.num_pts : static_cast<int>(bp / p.d.num_pts);
-        bool gate = false;
-        if (lane < npair) {
-            PairSetup ps;
-            gate = pair_setup(p.d, p.loc, lh, lw, ls, bp, my_cam, my_lv, ps);
-            mine[lane] = ps;
-        }
-        const uint32_t visible = __ballot_sync(0xffffffffu, gate);
-        __syncwarp();
+        const uint32_t visible = setup_pairs(p.d, p.loc, lh, lw, ls, bp, lane, my_cam, my_lv, nullptr, mine);
         const float *featb = p.feat + static_cast<long long>(b) * M * F * C;
+        float *gfeatb = p.grad_feat + static_cast<long long>(b) * M * F * C;
         const float *wpt = p.weights + bp * npair * Gr;
         for (int c0 = lane * 4; c0 < C; c0 += 128) {
             const int grp = c0 / gdim;
             float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
             float4 gout = make_float4(0.f, 0.f, 0.f, 0.f);
             if (BACKWARD) gout = __ldg(reinterpret_cast<const float4 *>(p.grad_out + bp * C + c0));
-            float gx = 0.f, gy = 0.f;
-            uint32_t todo = visible;
-            while (todo) {
-                const int pr = __ffs(todo) - 1;
-                todo &= todo - 1;
-                const int4 rows = *reinterpret_cast<const int4 *>(mine[pr].row);      // warp-uniform loads
-                const float4 cw = *reinterpret_cast<const float4 *>(mine[pr].w);
-                const float wt = __ldg(wpt + pr * Gr + grp);
-                const float4 v0 = __ldg(reinterpret_cast<const float4 *>(featb + rows.x + c0));
-                const float4 v1 = __ldg(reinterpret_cast<const float4 *>(featb + rows.y + c0));
-                const float4 v2 = __ldg(reinterpret_cast<const float4 *>(featb + rows.z + c0));
-                const float4 v3 = __ldg(reinterpret_cast<const float4 *>(featb + rows.w + c0));
-                if (!BACKWARD) {
-                    const float a0 = cw.x * wt, a1 = cw.y * wt, a2 = cw.z * wt, a3 = cw.w * wt;
-                    acc.x = fmaf(a0, v0.x, acc.x); acc.y = fmaf(a0, v0.y, acc.y); acc.z = fmaf(a0, v0.z, acc.z); acc.w = fmaf(a0, v0.w, acc.w);
-                    acc.x = fmaf(a1, v1.x, acc.x); acc.y = fmaf(a1, v1.y, acc.y); acc.z = fmaf(a1, v1.z, acc.z); acc.w = fmaf(a1, v1.w, acc.w);
-                    acc.x = fmaf(a2, v2.x, acc.x); acc.y = fmaf(a2, v2.y, acc.y); acc.z = fmaf(a2, v2.z, acc.z); acc.w = fmaf(a2, v2.w, acc.w);
-                    acc.x = fmaf(a3, v3.x, acc.x); acc.y = fmaf(a3, v3.y, acc.y); acc.z = fmaf(a3, v3.z, acc.z); acc.w = fmaf(a3, v3.w, acc.w);
-                } else {
-                    const float4 fr = *reinterpret_cast<const float4 *>(&mine[pr].lh);
-                    const int2 okcam = *reinterpret_cast<const int2 *>(&mine[pr].ok);
-                    const float2 frac = make_float2(fr.x, fr.y), dims = make_float2(fr.z, fr.w);
-                    const int ok = okcam.x;
-                    // d(out)/d(feat corner) = corner weight * aggregation weight, for corners inside the map
-                    float *gfb = p.grad_feat + static_cast<long long>(b) * M * F * C + c0;
-                    if (ok & 1) atomicAdd(reinterpret_cast<float4 *>(gfb + rows.x), make_float4(cw.x * wt * gout.x, cw.x * wt * gout.y, cw.x * wt * gout.z, cw.x * wt * gout.w));
-                    if (ok & 2) atomicAdd(reinterpret_cast<float4 *>(gfb + rows.y), make_float4(cw.y * wt * gout.x, cw.y * wt * gout.y, cw.y * wt * gout.z, cw.y * wt * gout.w));
-                    if (ok & 4) atomicAdd(reinterpret_cast<float4 *>(gfb + rows.z), make_float4(cw.z * wt * gout.x, cw.z * wt * gout.y, cw.z * wt * gout.z, cw.z * wt * gout.w));
-                    if (ok & 8) atomicAdd(reinterpret_cast<float4 *>(gfb + rows.w), make_float4(cw.w * wt * gout.x, cw.w * wt * gout.y, cw.w * wt * gout.z, cw.w * wt * gout.w));
-                    // g . v_k for the four corners (outside corners carry weight 0; their clamped values are masked below)
-                    const float m0 = (ok & 1) ? 1.f : 0.f, m1 = (ok & 2) ? 1.f : 0.f, m2 = (ok & 4) ? 1.f : 0.f, m3 = (ok & 8) ? 1.f : 0.f;
-                    const float d0 = m0 * (gout.x * v0.x + gout.y * v0.y + gout.z * v0.z + gout.w * v0.w);
-                    const float d1 = m1 * (gout.x * v1.x + gout.y * v1.y + gout.z * v1.z + gout.w * v1.w);
-                    const float d2 = m2 * (gout.x * v2.x + gout.y * v2.y + gout.z * v2.z + gout.w * v2.w);
-                    const float d3 = m3 * (gout.x * v3.x + gout.y * v3.y + gout.z * v3.z + gout.w * v3.w);
-                    const float lhh = frac.x, lww = frac.y, hh = 1.f - lhh, hw = 1.f - lww;
-                    // d(out)/d(weight) = sampled value . g   (cuda.cu:117-119)
-                    float gw = hh * hw * d0 + hh * lww * d1 + lhh * hw * d2 + lhh * lww * d3;
-                    // d(val)/d(x_im), d(val)/d(y_im)   (cuda.cu:85-121)
-                    gx = fmaf(dims.y * wt, -hh * d0 + hh * d1 - lhh * d2 + lhh * d3, gx);
-                    gy = fmaf(dims.x * wt, -hw * d0 - lww * d1 + hw * d2 + lww * d3, gy);
-                    const int lanes_per_group = gdim / 4;
-#pragma unroll
-                    for (int o = 1; o < 32; o <<= 1)
-                        if (o < lanes_per_group) gw += __shfl_xor_sync(0xffffffffu, gw, o);
-                    if ((lane & (lanes_per_group - 1)) == 0) p.grad_weights[(bp * npair + pr) * Gr + grp] += gw;
-                    // the location gradient of a camera is complete after its last visible level
-                    const int m = okcam.y;
-                    const bool cam_done = todo == 0 || mine[__ffs(todo) - 1].cam != m;
-                    if (cam_done) {
-#pragma unroll
-                        for (int o = 16; o > 0; o >>= 1) {
-                            gx += __shfl_xor_sync(0xffffffffu, gx, o);
-                            gy += __shfl_xor_sync(0xffffffffu, gy, o);
-                        }
-                        if (lane == 0) {
-                            float *gl = p.grad_loc + (bp * M + m) * 2;
-                            gl[0] += gx;
-                            gl[1] += gy;
-                        }
-                        gx = 0.f; gy = 0.f;
-                    }
-                }
-            }
+            visit_pairs<BACKWARD>(mine, visible, featb, gfeatb, c0, lane, lanes_per_group, gout, p.grad_loc, bp, M, acc,
+                                  [=](int pr) { return __ldg(wpt + pr * Gr + grp); },
+                                  [gwt = p.grad_weights, bp, npair, Gr, grp](int pr, float, float gw) { gwt[(bp * npair + pr) * Gr + grp] += gw; });
             if (!BACKWARD) *reinterpret_cast<float4 *>(p.out + bp * C + c0) = acc;
         }
         __syncwarp();   // the next point overwrites this warp's setup slots
     }
 }
 
-int launch_daf(const gf_daf_desc &d, const DafParams &dp, bool backward, int num_sms, cudaStream_t stream) {
-    const long long npts = static_cast<long long>(d.batch) * d.num_pts;
+int launch_daf(const DafParams &p, bool backward, int num_sms, cudaStream_t stream) {
+    const long long npts = static_cast<long long>(p.d.batch) * p.d.num_pts;
     if (npts == 0) return GF_OK;
-    const int per_cta = kDafThreads / 32;
-    long long want = (npts + per_cta - 1) / per_cta;
-    const long long cap = static_cast<long long>(num_sms) * 64;
-    const int grid = static_cast<int>(want < cap ? want : cap);
-    const bool v4 = daf_vec4_ok(d);
+    const int grid = daf_grid(npts, num_sms);
+    const bool v4 = daf_vec4_ok(p.d);
     if (backward) {
-        if (v4) daf_fast_kernel<true><<<grid, kDafThreads, 0, stream>>>(dp);
-        else daf_kernel<true><<<grid, kDafThreads, 0, stream>>>(dp);
+        if (v4) daf_fast_kernel<true><<<grid, kDafThreads, 0, stream>>>(p);
+        else daf_kernel<true><<<grid, kDafThreads, 0, stream>>>(p);
     } else {
-        if (v4) daf_fast_kernel<false><<<grid, kDafThreads, 0, stream>>>(dp);
-        else daf_kernel<false><<<grid, kDafThreads, 0, stream>>>(dp);
+        if (v4) daf_fast_kernel<false><<<grid, kDafThreads, 0, stream>>>(p);
+        else daf_kernel<false><<<grid, kDafThreads, 0, stream>>>(p);
     }
     GF_CUDA_TRY(cudaGetLastError());
     return GF_OK;
@@ -401,22 +303,6 @@ int launch_daf_format(const gf_daf_format_desc &d, float *const *maps, float *ta
     else daf_format_kernel<false><<<grid, 256, 0, stream>>>(fp);
     GF_CUDA_TRY(cudaGetLastError());
     return GF_OK;
-}
-
-int launch_daf_forward(const gf_daf_desc &d, const float *feat, const int32_t *shape, const int32_t *start,
-                       const float *loc, const float *weights, float *out, int num_sms, cudaStream_t stream) {
-    DafParams dp{};
-    dp.d = d; dp.feat = feat; dp.shape = shape; dp.start = start; dp.loc = loc; dp.weights = weights; dp.out = out;
-    return launch_daf(d, dp, false, num_sms, stream);
-}
-
-int launch_daf_backward(const gf_daf_desc &d, const float *feat, const int32_t *shape, const int32_t *start,
-                        const float *loc, const float *weights, const float *grad_out, float *grad_feat,
-                        float *grad_loc, float *grad_weights, int num_sms, cudaStream_t stream) {
-    DafParams dp{};
-    dp.d = d; dp.feat = feat; dp.shape = shape; dp.start = start; dp.loc = loc; dp.weights = weights;
-    dp.grad_out = grad_out; dp.grad_feat = grad_feat; dp.grad_loc = grad_loc; dp.grad_weights = grad_weights;
-    return launch_daf(d, dp, true, num_sms, stream);
 }
 
 }  // namespace gf

@@ -11,9 +11,9 @@
 //   pass 1/2  the warp reads the anchor's K*M*L*Gr raw logits once, coalesced (lane -> group lane % Gr),
 //             and keeps max and 1/sum per group: the normalised weight of an entry is then
 //             exp2(logit*log2e - max*log2e) / sum, evaluated where it is used and never stored;
-//   sampling  the K key points are visited in turn with the one-lane-per-(camera, level) setup of
-//             daf_fast_kernel (daf.cu); the accumulator stays in registers across key points and is
-//             written once per anchor ([B, A, C]: K times fewer output bytes).
+//   sampling  the K key points are visited in turn with the pair setup and visit of daf_fast_kernel
+//             (setup_pairs / visit_pairs, daf_pair.cuh); the accumulator stays in registers across key
+//             points and is written once per anchor ([B, A, C]: K times fewer output bytes).
 //
 // Backward uses  sum_e w_e * dL/dw_e = sum_{c in group} dL/dout_c * out_c  (out = sum_e w_e * val_e), so
 // the softmax gradient  w_e * (dL/dw_e - that sum)  needs no second pass over the samples: every entry first
@@ -23,35 +23,13 @@
 
 namespace gf {
 
-struct DafFusedParams {
-    gf_daf_desc d;
-    int K;                        // key points per anchor
-    const float *feat;
-    const int32_t *shape;
-    const int32_t *start;
-    const float *loc;             // [B, A*K, M, 2]
-    const float *logits;          // [B, A, K, M, L, Gr] raw (pre-softmax) weights
-    const uint8_t *pmask;         // [B, A, K, M] or NULL
-    const uint8_t *wmask;         // [B, A, K, M, L, Gr] or NULL
-    float *out;                   // forward:  [B, A, C]
-    float *stats;                 // forward writes / backward reads [B, A, Gr, 2] = (max*log2e, 1/sum)
-    const float *out_saved;       // backward: the forward output
-    const float *grad_out;        // backward: [B, A, C]
-    float *grad_feat, *grad_loc, *grad_logits;
-};
-
 template <bool BACKWARD>
 __global__ void __launch_bounds__(kDafThreads, BACKWARD ? 3 : 4) daf_fused_kernel(const DafFusedParams p) {
     constexpr int kWarps = kDafThreads / 32;
     __shared__ int lh[kMaxLevels], lw[kMaxLevels], ls[kMaxLevels];
     __shared__ __align__(16) PairSetup s_pair[kWarps][32];
     __shared__ float s_mlog[kWarps][32], s_inv[kWarps][32], s_dot[kWarps][32];
-    if (threadIdx.x < p.d.num_scale) {
-        lh[threadIdx.x] = p.shape[2 * threadIdx.x];
-        lw[threadIdx.x] = p.shape[2 * threadIdx.x + 1];
-        ls[threadIdx.x] = p.start[threadIdx.x];
-    }
-    __syncthreads();
+    load_level_table(p.d, p.shape, p.start, lh, lw, ls);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int C = p.d.num_embeds, M = p.d.num_cams, L = p.d.num_scale, Gr = p.d.num_groups, F = p.d.num_feat;
     const int K = p.K, npair = M * L, LG = L * Gr;
@@ -127,6 +105,7 @@ __global__ void __launch_bounds__(kDafThreads, BACKWARD ? 3 : 4) daf_fused_kerne
 
         // ---- sampling: K key points accumulate into one register vector per lane -----------------------------
         const float *featb = p.feat + static_cast<long long>(b) * M * F * C;
+        float *gfeatb = p.grad_feat + static_cast<long long>(b) * M * F * C;
         for (int c0 = lane * 4; c0 < C; c0 += 128) {
             const int grp = c0 / gdim;
             const float mlog = s_mlog[warp][grp], inv = s_inv[warp][grp];
@@ -136,80 +115,20 @@ __global__ void __launch_bounds__(kDafThreads, BACKWARD ? 3 : 4) daf_fused_kerne
             if (BACKWARD) gout = __ldg(reinterpret_cast<const float4 *>(p.grad_out + ba * C + c0));
             for (int k = 0; k < K; ++k) {
                 const long long bp = ba * K + k;
-                bool gate = false;
-                if (lane < npair) {
-                    PairSetup ps;
-                    gate = pair_setup(p.d, p.loc, lh, lw, ls, bp, my_cam, my_lv, ps);
-                    if (pm) gate = gate && pm[k * M + my_cam] != 0;    // a masked point has weight 0 in every level and group
-                    mine[lane] = ps;
-                }
-                const uint32_t visible = __ballot_sync(0xffffffffu, gate);
-                __syncwarp();
+                const uint32_t visible = setup_pairs(p.d, p.loc, lh, lw, ls, bp, lane, my_cam, my_lv, pm ? pm + k * M : nullptr, mine);
                 const float *wpt = wl + k * npair * Gr;
                 const uint8_t *wmk = wm ? wm + k * npair * Gr : nullptr;
-                float gx = 0.f, gy = 0.f;
-                uint32_t todo = visible;
-                while (todo) {
-                    const int pr = __ffs(todo) - 1;
-                    todo &= todo - 1;
-                    const int4 rows = *reinterpret_cast<const int4 *>(mine[pr].row);      // warp-uniform loads
-                    const float4 cw = *reinterpret_cast<const float4 *>(mine[pr].w);
-                    const int widx = pr * Gr + grp;
-                    float wt = ex2_approx(fmaf(__ldg(wpt + widx), kLog2e, -mlog)) * inv;
-                    if (wmk && !wmk[widx]) wt = 0.f;                                  // select, never multiply: a masked logit may be anything
-                    const float4 v0 = __ldg(reinterpret_cast<const float4 *>(featb + rows.x + c0));
-                    const float4 v1 = __ldg(reinterpret_cast<const float4 *>(featb + rows.y + c0));
-                    const float4 v2 = __ldg(reinterpret_cast<const float4 *>(featb + rows.z + c0));
-                    const float4 v3 = __ldg(reinterpret_cast<const float4 *>(featb + rows.w + c0));
-                    if (!BACKWARD) {
-                        const float a0 = cw.x * wt, a1 = cw.y * wt, a2 = cw.z * wt, a3 = cw.w * wt;
-                        acc.x = fmaf(a0, v0.x, acc.x); acc.y = fmaf(a0, v0.y, acc.y); acc.z = fmaf(a0, v0.z, acc.z); acc.w = fmaf(a0, v0.w, acc.w);
-                        acc.x = fmaf(a1, v1.x, acc.x); acc.y = fmaf(a1, v1.y, acc.y); acc.z = fmaf(a1, v1.z, acc.z); acc.w = fmaf(a1, v1.w, acc.w);
-                        acc.x = fmaf(a2, v2.x, acc.x); acc.y = fmaf(a2, v2.y, acc.y); acc.z = fmaf(a2, v2.z, acc.z); acc.w = fmaf(a2, v2.w, acc.w);
-                        acc.x = fmaf(a3, v3.x, acc.x); acc.y = fmaf(a3, v3.y, acc.y); acc.z = fmaf(a3, v3.z, acc.z); acc.w = fmaf(a3, v3.w, acc.w);
-                    } else {
-                        const float4 fr = *reinterpret_cast<const float4 *>(&mine[pr].lh);
-                        const int2 okcam = *reinterpret_cast<const int2 *>(&mine[pr].ok);
-                        const int ok = okcam.x;
-                        // d(out)/d(feat corner) = corner weight * normalised aggregation weight (corners inside the map)
-                        float *gfb = p.grad_feat + static_cast<long long>(b) * M * F * C + c0;
-                        if (ok & 1) atomicAdd(reinterpret_cast<float4 *>(gfb + rows.x), make_float4(cw.x * wt * gout.x, cw.x * wt * gout.y, cw.x * wt * gout.z, cw.x * wt * gout.w));
-                        if (ok & 2) atomicAdd(reinterpret_cast<float4 *>(gfb + rows.y), make_float4(cw.y * wt * gout.x, cw.y * wt * gout.y, cw.y * wt * gout.z, cw.y * wt * gout.w));
-                        if (ok & 4) atomicAdd(reinterpret_cast<float4 *>(gfb + rows.z), make_float4(cw.z * wt * gout.x, cw.z * wt * gout.y, cw.z * wt * gout.z, cw.z * wt * gout.w));
-                        if (ok & 8) atomicAdd(reinterpret_cast<float4 *>(gfb + rows.w), make_float4(cw.w * wt * gout.x, cw.w * wt * gout.y, cw.w * wt * gout.z, cw.w * wt * gout.w));
-                        const float m0 = (ok & 1) ? 1.f : 0.f, m1 = (ok & 2) ? 1.f : 0.f, m2 = (ok & 4) ? 1.f : 0.f, m3 = (ok & 8) ? 1.f : 0.f;
-                        const float d0 = m0 * (gout.x * v0.x + gout.y * v0.y + gout.z * v0.z + gout.w * v0.w);
-                        const float d1 = m1 * (gout.x * v1.x + gout.y * v1.y + gout.z * v1.z + gout.w * v1.w);
-                        const float d2 = m2 * (gout.x * v2.x + gout.y * v2.y + gout.z * v2.z + gout.w * v2.w);
-                        const float d3 = m3 * (gout.x * v3.x + gout.y * v3.y + gout.z * v3.z + gout.w * v3.w);
-                        const float lhh = fr.x, lww = fr.y, hh = 1.f - lhh, hw = 1.f - lww;
-                        // dL/dw_e = sampled value . g  (deformable_aggregation_cuda.cu:117-119), then through the softmax
-                        float gw = hh * hw * d0 + hh * lww * d1 + lhh * hw * d2 + lhh * lww * d3;
-                        gx = fmaf(fr.w * wt, -hh * d0 + hh * d1 - lhh * d2 + lhh * d3, gx);
-                        gy = fmaf(fr.z * wt, -hw * d0 - lww * d1 + hw * d2 + lww * d3, gy);
-#pragma unroll
-                        for (int o = 1; o < 32; o <<= 1)
-                            if (o < lanes_per_group) gw += __shfl_xor_sync(0xffffffffu, gw, o);
-                        if ((lane & (lanes_per_group - 1)) == 0)
-                            p.grad_logits[ba * nE + static_cast<long long>(k) * npair * Gr + widx] = wt * (gw - S);
-                        // the location gradient of a camera is complete after its last visible level
-                        const int m = okcam.y;
-                        const bool cam_done = todo == 0 || mine[__ffs(todo) - 1].cam != m;
-                        if (cam_done) {
-#pragma unroll
-                            for (int o = 16; o > 0; o >>= 1) {
-                                gx += __shfl_xor_sync(0xffffffffu, gx, o);
-                                gy += __shfl_xor_sync(0xffffffffu, gy, o);
-                            }
-                            if (lane == 0) {
-                                float *gl = p.grad_loc + (bp * M + m) * 2;
-                                gl[0] += gx;
-                                gl[1] += gy;
-                            }
-                            gx = 0.f; gy = 0.f;
-                        }
-                    }
-                }
+                visit_pairs<BACKWARD>(
+                    mine, visible, featb, gfeatb, c0, lane, lanes_per_group, gout, p.grad_loc, bp, M, acc,
+                    [=](int pr) {
+                        const int widx = pr * Gr + grp;
+                        const float wt = ex2_approx(fmaf(__ldg(wpt + widx), kLog2e, -mlog)) * inv;
+                        return (wmk && !wmk[widx]) ? 0.f : wt;       // select, never multiply: a masked logit may be anything
+                    },
+                    // dL/dw_e = sampled value . g, then through the softmax
+                    [glg = p.grad_logits, ba, nE, k, npair, Gr, grp, S](int pr, float wt, float gw) {
+                        glg[ba * nE + static_cast<long long>(k) * npair * Gr + pr * Gr + grp] = wt * (gw - S);
+                    });
                 __syncwarp();   // the next key point overwrites this warp's setup slots
             }
             if (!BACKWARD) *reinterpret_cast<float4 *>(p.out + ba * C + c0) = acc;
@@ -226,37 +145,14 @@ bool daf_fused_supported(const gf_daf_desc &d, int K) {
     return static_cast<long long>(K) * d.num_cams * d.num_scale * Gr < (1ll << 31);
 }
 
-static int launch_daf_fused(const DafFusedParams &fp, bool backward, int num_sms, cudaStream_t stream) {
-    const long long nanchor = static_cast<long long>(fp.d.batch) * (fp.d.num_pts / fp.K);
+int launch_daf_fused(const DafFusedParams &p, bool backward, int num_sms, cudaStream_t stream) {
+    const long long nanchor = static_cast<long long>(p.d.batch) * (p.d.num_pts / p.K);
     if (nanchor == 0) return GF_OK;
-    const int per_cta = kDafThreads / 32;
-    const long long want = (nanchor + per_cta - 1) / per_cta;
-    const long long cap = static_cast<long long>(num_sms) * 64;
-    const int grid = static_cast<int>(want < cap ? want : cap);
-    if (backward) daf_fused_kernel<true><<<grid, kDafThreads, 0, stream>>>(fp);
-    else daf_fused_kernel<false><<<grid, kDafThreads, 0, stream>>>(fp);
+    const int grid = daf_grid(nanchor, num_sms);
+    if (backward) daf_fused_kernel<true><<<grid, kDafThreads, 0, stream>>>(p);
+    else daf_fused_kernel<false><<<grid, kDafThreads, 0, stream>>>(p);
     GF_CUDA_TRY(cudaGetLastError());
     return GF_OK;
-}
-
-int launch_daf_fused_forward(const gf_daf_desc &d, int K, const float *feat, const int32_t *shape, const int32_t *start,
-                             const float *loc, const float *logits, const uint8_t *pmask, const uint8_t *wmask,
-                             float *out, float *stats, int num_sms, cudaStream_t stream) {
-    DafFusedParams fp{};
-    fp.d = d; fp.K = K; fp.feat = feat; fp.shape = shape; fp.start = start; fp.loc = loc; fp.logits = logits;
-    fp.pmask = pmask; fp.wmask = wmask; fp.out = out; fp.stats = stats;
-    return launch_daf_fused(fp, false, num_sms, stream);
-}
-
-int launch_daf_fused_backward(const gf_daf_desc &d, int K, const float *feat, const int32_t *shape, const int32_t *start,
-                              const float *loc, const float *logits, const uint8_t *pmask, const uint8_t *wmask,
-                              const float *stats, const float *out, const float *grad_out, float *grad_feat,
-                              float *grad_loc, float *grad_logits, int num_sms, cudaStream_t stream) {
-    DafFusedParams fp{};
-    fp.d = d; fp.K = K; fp.feat = feat; fp.shape = shape; fp.start = start; fp.loc = loc; fp.logits = logits;
-    fp.pmask = pmask; fp.wmask = wmask; fp.stats = const_cast<float *>(stats); fp.out_saved = out; fp.grad_out = grad_out;
-    fp.grad_feat = grad_feat; fp.grad_loc = grad_loc; fp.grad_logits = grad_logits;
-    return launch_daf_fused(fp, true, num_sms, stream);
 }
 
 }  // namespace gf

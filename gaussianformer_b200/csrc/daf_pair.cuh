@@ -1,5 +1,13 @@
-// Pieces shared by the deformable-aggregation kernels (daf.cu, daf_fused.cu): the per-(camera, level)
-// bilinear setup that one lane computes for its whole warp.
+// Pieces shared by the deformable-aggregation kernels (daf.cu, daf_fused.cu): their launch parameters, the level
+// table, and the one-warp-per-point visit of the fast kernels (daf_fast_kernel, daf_fused_kernel):
+//   lane p < M*L      : pair p = (camera p / L, level p % L): gate, 4 corner rows (clamped to a valid row), 4 corner
+//                       weights (zero for corners outside the map) -> per-warp smem          (setup_pairs)
+//   ballot of the gate: only visible pairs are visited, in ascending (camera, level) order   (visit_pairs)
+//   every visit       : 2-3 uniform LDS.128 for the setup, one weight, 4 coalesced 16-byte row loads per lane,
+//                       16 FMAs
+//   backward          : 16-byte vector atomics for the feature gradient, the weight gradient reduced over the lanes
+//                       of a group with shuffles and handed to one lane, the location gradient reduced over the warp
+//                       once per visible camera
 #pragma once
 #include "common.cuh"
 
@@ -7,6 +15,35 @@ namespace gf {
 
 constexpr int kDafThreads = 256;
 constexpr int kMaxLevels = 8;
+
+struct DafParams {
+    gf_daf_desc d;
+    const float *feat;
+    const int32_t *shape;
+    const int32_t *start;
+    const float *loc;
+    const float *weights;
+    float *out;               // forward
+    const float *grad_out;    // backward
+    float *grad_feat, *grad_loc, *grad_weights;
+};
+
+struct DafFusedParams {
+    gf_daf_desc d;
+    int K;                        // key points per anchor
+    const float *feat;
+    const int32_t *shape;
+    const int32_t *start;
+    const float *loc;             // [B, A*K, M, 2]
+    const float *logits;          // [B, A, K, M, L, Gr] raw (pre-softmax) weights
+    const uint8_t *pmask;         // [B, A, K, M] or NULL
+    const uint8_t *wmask;         // [B, A, K, M, L, Gr] or NULL
+    float *out;                   // forward:  [B, A, C]
+    float *stats;                 // forward writes / backward reads [B, A, Gr, 2] = (max*log2e, 1/sum)
+    const float *out_saved;       // backward: the forward output
+    const float *grad_out;        // backward: [B, A, C]
+    float *grad_feat, *grad_loc, *grad_logits;
+};
 
 struct PairSetup {     // 64 bytes per (camera, level) pair
     int row[4];        // element offset of each corner row inside the batch's feature block (row * C)
@@ -17,6 +54,18 @@ struct PairSetup {     // 64 bytes per (camera, level) pair
     int cam;           // camera of this pair
     int pad0, pad1;
 };
+
+// Level table into shared memory (dynamically indexed registers would spill to local memory); ends with a
+// __syncthreads, so every thread of the block must call it.
+__device__ __forceinline__ void load_level_table(const gf_daf_desc &d, const int32_t *shape, const int32_t *start,
+                                                 int *lh, int *lw, int *ls) {
+    if (threadIdx.x < d.num_scale) {
+        lh[threadIdx.x] = shape[2 * threadIdx.x];
+        lw[threadIdx.x] = shape[2 * threadIdx.x + 1];
+        ls[threadIdx.x] = start[threadIdx.x];
+    }
+    __syncthreads();
+}
 
 __device__ __forceinline__ bool pair_setup(const gf_daf_desc &d, const float *loc, const int *lh, const int *lw, const int *ls,
                                            long long bp, int m, int lv, PairSetup &o) {
@@ -47,6 +96,100 @@ __device__ __forceinline__ bool pair_setup(const gf_daf_desc &d, const float *lo
     return gate;
 }
 
+// Setup of sampling point bp: lane p < M*L writes the setup of its pair (my_cam, my_lv) into the warp's slots.
+// Returns the ballot of the pairs whose camera sees the point and, with a point-mask row pm ([M] or nullptr),
+// whose pm[camera] is set.  The whole warp must call it; the slots are complete on return.
+__device__ __forceinline__ uint32_t setup_pairs(const gf_daf_desc &d, const float *loc, const int *lh, const int *lw,
+                                                const int *ls, long long bp, int lane, int my_cam, int my_lv,
+                                                const uint8_t *pm, PairSetup *mine) {
+    bool gate = false;
+    if (lane < d.num_cams * d.num_scale) {
+        PairSetup ps;
+        gate = pair_setup(d, loc, lh, lw, ls, bp, my_cam, my_lv, ps);
+        if (pm) gate = gate && pm[my_cam] != 0;    // a masked point has weight 0 in every level and group
+        mine[lane] = ps;
+    }
+    const uint32_t visible = __ballot_sync(0xffffffffu, gate);
+    __syncwarp();
+    return visible;
+}
+
+// Visits the visible pairs of one sampling point for the channel slice [c0, c0 + 4) of this lane.
+//   featb / gfeatb : feature table and feature gradient of the point's batch
+//   grad_loc, bp, M: location gradient and the point's index; the row address (bp * M + camera) * 2 is formed
+//                    only where the row is written, so no pointer stays live across the visit (backward)
+//   weight(pr)     : aggregation weight of pair pr for this lane's group
+//   weight_grad(pr, wt, gw) : called by the first lane of each group with the group's dL/d(weight) of pair pr
+// Forward accumulates into acc; backward leaves acc alone.  The callers' callables capture by value: capturing
+// the kernel's locals by reference compiles the plain backward to a different register allocation.
+template <bool BACKWARD, class Weight, class WeightGrad>
+__device__ __forceinline__ void visit_pairs(const PairSetup *mine, uint32_t visible, const float *featb, float *gfeatb,
+                                            int c0, int lane, int lanes_per_group, float4 gout, float *grad_loc,
+                                            long long bp, int M, float4 &acc, Weight weight, WeightGrad weight_grad) {
+    float gx = 0.f, gy = 0.f;
+    uint32_t todo = visible;
+    while (todo) {
+        const int pr = __ffs(todo) - 1;
+        todo &= todo - 1;
+        const int4 rows = *reinterpret_cast<const int4 *>(mine[pr].row);      // warp-uniform loads
+        const float4 cw = *reinterpret_cast<const float4 *>(mine[pr].w);
+        const float wt = weight(pr);
+        const float4 v0 = __ldg(reinterpret_cast<const float4 *>(featb + rows.x + c0));
+        const float4 v1 = __ldg(reinterpret_cast<const float4 *>(featb + rows.y + c0));
+        const float4 v2 = __ldg(reinterpret_cast<const float4 *>(featb + rows.z + c0));
+        const float4 v3 = __ldg(reinterpret_cast<const float4 *>(featb + rows.w + c0));
+        if (!BACKWARD) {
+            const float a0 = cw.x * wt, a1 = cw.y * wt, a2 = cw.z * wt, a3 = cw.w * wt;
+            acc.x = fmaf(a0, v0.x, acc.x); acc.y = fmaf(a0, v0.y, acc.y); acc.z = fmaf(a0, v0.z, acc.z); acc.w = fmaf(a0, v0.w, acc.w);
+            acc.x = fmaf(a1, v1.x, acc.x); acc.y = fmaf(a1, v1.y, acc.y); acc.z = fmaf(a1, v1.z, acc.z); acc.w = fmaf(a1, v1.w, acc.w);
+            acc.x = fmaf(a2, v2.x, acc.x); acc.y = fmaf(a2, v2.y, acc.y); acc.z = fmaf(a2, v2.z, acc.z); acc.w = fmaf(a2, v2.w, acc.w);
+            acc.x = fmaf(a3, v3.x, acc.x); acc.y = fmaf(a3, v3.y, acc.y); acc.z = fmaf(a3, v3.z, acc.z); acc.w = fmaf(a3, v3.w, acc.w);
+        } else {
+            const float4 fr = *reinterpret_cast<const float4 *>(&mine[pr].lh);
+            const int2 okcam = *reinterpret_cast<const int2 *>(&mine[pr].ok);
+            const int ok = okcam.x;
+            // d(out)/d(feat corner) = corner weight * aggregation weight, for corners inside the map
+            float *gfb = gfeatb + c0;
+            if (ok & 1) atomicAdd(reinterpret_cast<float4 *>(gfb + rows.x), make_float4(cw.x * wt * gout.x, cw.x * wt * gout.y, cw.x * wt * gout.z, cw.x * wt * gout.w));
+            if (ok & 2) atomicAdd(reinterpret_cast<float4 *>(gfb + rows.y), make_float4(cw.y * wt * gout.x, cw.y * wt * gout.y, cw.y * wt * gout.z, cw.y * wt * gout.w));
+            if (ok & 4) atomicAdd(reinterpret_cast<float4 *>(gfb + rows.z), make_float4(cw.z * wt * gout.x, cw.z * wt * gout.y, cw.z * wt * gout.z, cw.z * wt * gout.w));
+            if (ok & 8) atomicAdd(reinterpret_cast<float4 *>(gfb + rows.w), make_float4(cw.w * wt * gout.x, cw.w * wt * gout.y, cw.w * wt * gout.z, cw.w * wt * gout.w));
+            // g . v_k for the four corners (outside corners carry weight 0; their clamped values are masked below)
+            const float m0 = (ok & 1) ? 1.f : 0.f, m1 = (ok & 2) ? 1.f : 0.f, m2 = (ok & 4) ? 1.f : 0.f, m3 = (ok & 8) ? 1.f : 0.f;
+            const float d0 = m0 * (gout.x * v0.x + gout.y * v0.y + gout.z * v0.z + gout.w * v0.w);
+            const float d1 = m1 * (gout.x * v1.x + gout.y * v1.y + gout.z * v1.z + gout.w * v1.w);
+            const float d2 = m2 * (gout.x * v2.x + gout.y * v2.y + gout.z * v2.z + gout.w * v2.w);
+            const float d3 = m3 * (gout.x * v3.x + gout.y * v3.y + gout.z * v3.z + gout.w * v3.w);
+            const float lhh = fr.x, lww = fr.y, hh = 1.f - lhh, hw = 1.f - lww;
+            // d(out)/d(weight) = sampled value . g   (deformable_aggregation_cuda.cu:117-119)
+            float gw = hh * hw * d0 + hh * lww * d1 + lhh * hw * d2 + lhh * lww * d3;
+            // d(val)/d(x_im), d(val)/d(y_im)   (deformable_aggregation_cuda.cu:85-121)
+            gx = fmaf(fr.w * wt, -hh * d0 + hh * d1 - lhh * d2 + lhh * d3, gx);
+            gy = fmaf(fr.z * wt, -hw * d0 - lww * d1 + hw * d2 + lww * d3, gy);
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1)
+                if (o < lanes_per_group) gw += __shfl_xor_sync(0xffffffffu, gw, o);
+            if ((lane & (lanes_per_group - 1)) == 0) weight_grad(pr, wt, gw);
+            // the location gradient of a camera is complete after its last visible level
+            const int m = okcam.y;
+            const bool cam_done = todo == 0 || mine[__ffs(todo) - 1].cam != m;
+            if (cam_done) {
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) {
+                    gx += __shfl_xor_sync(0xffffffffu, gx, o);
+                    gy += __shfl_xor_sync(0xffffffffu, gy, o);
+                }
+                if (lane == 0) {
+                    float *gl = grad_loc + (bp * M + m) * 2;
+                    gl[0] += gx;
+                    gl[1] += gy;
+                }
+                gx = 0.f; gy = 0.f;
+            }
+        }
+    }
+}
+
 // conditions of the one-warp-per-point fast kernels: C % 128 == 0, a group = a power-of-two run of whole
 // lanes, at most 32 (camera, level) pairs, 32-bit row offsets
 inline bool daf_vec4_ok(const gf_daf_desc &d) {
@@ -57,6 +200,15 @@ inline bool daf_vec4_ok(const gf_daf_desc &d) {
     if (gdim % 4 != 0) return false;
     const int lpg = gdim / 4;
     return lpg <= 32 && (lpg & (lpg - 1)) == 0;
+}
+
+// CTAs for `items` warp-sized work items (points or anchors): one warp each, at most 64 CTAs per SM; the kernels
+// loop over what does not fit
+inline int daf_grid(long long items, int num_sms) {
+    const int per_cta = kDafThreads / 32;
+    const long long want = (items + per_cta - 1) / per_cta;
+    const long long cap = static_cast<long long>(num_sms) * 64;
+    return static_cast<int>(want < cap ? want : cap);
 }
 
 }  // namespace gf

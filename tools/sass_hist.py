@@ -8,7 +8,8 @@ KERNELS = [("render_tile_kernel<18,false>", "_ZN2gf18render_tile_kernelILi18ELb0
            ("backward_bin_kernel<18,false>", "backward_bin_kernelILi18ELb0"),
            ("backward_bin_kernel<18,true>", "backward_bin_kernelILi18ELb1"),
            ("pack_mask_kernel", "pack_mask_kernel"), ("list_kernel", "list_kernel"),
-           ("daf_fast_kernel<fwd>", "daf_fast_kernelILb0")]
+           ("daf_fast_kernel<fwd>", "daf_fast_kernelILb0"), ("daf_fast_kernel<bwd>", "daf_fast_kernelILb1"),
+           ("daf_fused_kernel<fwd>", "daf_fused_kernelILb0"), ("daf_fused_kernel<bwd>", "daf_fused_kernelILb1")]
 sass = subprocess.run(["cuobjdump", "-sass", LIB], capture_output=True, text=True).stdout
 funcs, cur = {}, None
 for line in sass.splitlines():
