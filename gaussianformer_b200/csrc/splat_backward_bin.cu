@@ -100,6 +100,34 @@ __device__ __forceinline__ int small_div(int i, int n) {
     return static_cast<int>((static_cast<uint32_t>(i) * kRcp16[n]) >> 16);
 }
 
+// Waits for the bin's tiles, then checks the canonical order of its points (point n must lie in voxel n): the bin
+// kernel assumed it; a violation clears the flag, bin_finish_kernel then discards the sums and the Gaussian-centric
+// kernels (which build the voxel -> point map) produce the gradients instead.
+template <int C, bool PROB>
+__device__ __forceinline__ void check_bin_order(const BwdParams &p, BinSmem<C, PROB> &sm, int binX0, int binY0, int binZ0) {
+    constexpr int NT = kBinThreads;
+    const int tid = threadIdx.x, H = p.d.H, W = p.d.W, D = p.d.D;
+    mbar_wait(&sm.bar, 0);
+#pragma unroll
+    for (int r = 0; r < 512 / NT; ++r) {
+        const int i = tid + r * NT, col = i >> 4, z = i & 15;
+        const int X = binX0 + (col >> 2), Y = binY0 + (col & 3), Z = binZ0 + z;
+        if (X < H && Y < W && Z < D) {
+            int vx, vy, vz;
+            if (p.in.points_int) {
+                const long long n = (static_cast<long long>(X) * W + Y) * D + Z;
+                vx = p.in.points_int[3 * n]; vy = p.in.points_int[3 * n + 1]; vz = p.in.points_int[3 * n + 2];
+            } else {
+                const float *pp = &sm.pts[col * (kBinZ * 3) + z * 3];
+                vx = voxel_coord(pp[0], p.d.pc_min[0], p.d.grid_size);
+                vy = voxel_coord(pp[1], p.d.pc_min[1], p.d.grid_size);
+                vz = voxel_coord(pp[2], p.d.pc_min[2], p.d.grid_size);
+            }
+            if (vx != X || vy != Y || vz != Z) *p.canon = 0;   // benign race: every writer stores 0
+        }
+    }
+}
+
 template <int C, bool PROB>
 __global__ void __launch_bounds__(kBinThreads, 2) backward_bin_kernel(const BwdParams pb, const BinParams bp,
                                                                        const __grid_constant__ BinMaps maps) {
@@ -109,7 +137,7 @@ __global__ void __launch_bounds__(kBinThreads, 2) backward_bin_kernel(const BwdP
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int sample = blockIdx.z / bp.nbx;
     const BwdParams p = sample_bwd(pb, sample);
-    const int H = p.d.H, W = p.d.W, D = p.d.D;
+    const int H = p.d.H;
     const int binX0 = (blockIdx.z - sample * bp.nbx) * kBinX, binY0 = blockIdx.y * kBinY, binZ0 = blockIdx.x * kBinZ;
     if (tid == 0) {
         mbar_init(&sm.bar, 1);
@@ -134,6 +162,12 @@ __global__ void __launch_bounds__(kBinThreads, 2) backward_bin_kernel(const BwdP
     const int s = sample * bp.nsuper + (binX0 >> st_shift) * bp.nsy + (binY0 >> st_shift);
     const int ncand = bp.counts[s];
     const PackedBox *boxes = bp.boxes + static_cast<size_t>(sample) * p.d.G;
+    if (ncand == 0) {
+        // No Gaussian to walk, but the point order is still this bin's to check: a point stored here may lie in a
+        // covered voxel (several points in one voxel).  Waiting also keeps the CTA from exiting with its copies in flight.
+        check_bin_order<C, PROB>(p, sm, binX0, binY0, binZ0);
+        return;
+    }
     bool tiles_ready = false;
 
     int cpos = 0;
@@ -181,29 +215,8 @@ __global__ void __launch_bounds__(kBinThreads, 2) backward_bin_kernel(const BwdP
             if (i < nlist) sm.sorted[atomicAdd(&sm.hist[mykey[r]], 1)] = sm.list[i];
         }
         if (!tiles_ready) {   // the tiles were in flight during the first Phase A
-            mbar_wait(&sm.bar, 0);
+            check_bin_order<C, PROB>(p, sm, binX0, binY0, binZ0);
             tiles_ready = true;
-            // canonical-order check of MY bin's points (point n must lie in voxel n): this kernel assumed it; a
-            // violation clears the flag, bin_finish_kernel then discards the sums and the Gaussian-centric kernels
-            // (which build the voxel -> point map) produce the gradients instead
-#pragma unroll
-            for (int r = 0; r < 512 / NT; ++r) {
-                const int i = tid + r * NT, col = i >> 4, z = i & 15;
-                const int X = binX0 + (col >> 2), Y = binY0 + (col & 3), Z = binZ0 + z;
-                if (X < H && Y < W && Z < D) {
-                    int vx, vy, vz;
-                    if (p.in.points_int) {
-                        const long long n = (static_cast<long long>(X) * W + Y) * D + Z;
-                        vx = p.in.points_int[3 * n]; vy = p.in.points_int[3 * n + 1]; vz = p.in.points_int[3 * n + 2];
-                    } else {
-                        const float *pp = &sm.pts[col * (kBinZ * 3) + z * 3];
-                        vx = voxel_coord(pp[0], p.d.pc_min[0], p.d.grid_size);
-                        vy = voxel_coord(pp[1], p.d.pc_min[1], p.d.grid_size);
-                        vz = voxel_coord(pp[2], p.d.pc_min[2], p.d.grid_size);
-                    }
-                    if (vx != X || vy != Y || vz != Z) *p.canon = 0;   // benign race: every writer stores 0
-                }
-            }
         }
         __syncthreads();
 

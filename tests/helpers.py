@@ -118,13 +118,14 @@ def oracle_grads(kw, inp, variant, grads, saved_from=None):
     return out
 
 
-def check_module_grads(t, kw, inp, variant, grads, what="", saved_from=None, golden=None):
-    """Gradients accumulated on the leaf tensors ``t`` (sample 0) against the oracle with assert_grad_parity.
+def check_module_grads(t, kw, inp, variant, grads, what="", saved_from=None, golden=None, sample=0):
+    """Gradients accumulated on the leaf tensors ``t`` (batch entry ``sample``; ``inp`` holds that sample alone)
+    against the oracle with assert_grad_parity.
     ``golden``: optional dict of reference-op gradients (same keys): the new op is also compared with it, the
     slack being the golden's own measured distance from the fp64 oracle."""
     g64, g32 = oracle_grads(kw, inp, variant, grads, saved_from)
     for name in ("means", "opa", "sem", "cov"):
-        mine = t[name].grad[0].detach().cpu().numpy()
+        mine = t[name].grad[sample].detach().cpu().numpy()
         assert_grad_parity(mine, g64[name], g32[name], what=f"{what} grad {name}")
         if golden is not None:
             gold = np.asarray(golden[name], np.float64)

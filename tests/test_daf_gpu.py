@@ -29,14 +29,17 @@ def _run(fms, loc, w, backward_seed=None):
     return feat, shape, start, out, grads
 
 
-@pytest.mark.parametrize("embed,groups,levels", [
-    (128, 4, ((12, 20), (6, 10), (3, 5))),        # vectorised path (C % 128 == 0)
-    (256, 8, ((9, 7), (5, 4))),                   # two channel slices per warp
-    (16, 4, ((7, 12), (4, 6), (2, 3))),           # scalar fallback path
-    (24, 3, ((5, 5),)),
+@pytest.mark.parametrize("embed,groups,levels,cams", [
+    (128, 4, ((12, 20), (6, 10), (3, 5)), 3),     # vectorised path (C % 128 == 0)
+    (256, 8, ((9, 7), (5, 4)), 3),                # two channel slices per warp
+    (16, 4, ((7, 12), (4, 6), (2, 3)), 3),        # scalar fallback path
+    (24, 3, ((5, 5),), 3),
+    # C = 128 on the general kernel: 6 cameras x 6 levels = 36 (camera, level) pairs, more than a warp's lanes
+    (128, 4, ((10, 16), (8, 12), (6, 9), (4, 6), (3, 4), (2, 2)), 6),
+    (128, 64, ((12, 20), (6, 10), (3, 5)), 3),    # C = 128 on the general kernel: 2 channels per group
 ])
-def test_daf_forward_backward_vs_oracle(embed, groups, levels):
-    fms, loc, w = make_daf_inputs(num_anchor=64, num_pts=5, batch=2, num_cams=3, embed_dims=embed,
+def test_daf_forward_backward_vs_oracle(embed, groups, levels, cams):
+    fms, loc, w = make_daf_inputs(num_anchor=64, num_pts=5, batch=2, num_cams=cams, embed_dims=embed,
                                   num_groups=groups, levels=levels, visible_p=0.5, seed=3)
     loc[0, 0, 0] = torch.tensor([0.0, 0.5]); loc[0, 1, 0] = torch.tensor([1.0, 0.5])
     loc[0, 2, 0] = torch.tensor([0.004, 0.996]); loc[0, 3, 1] = torch.tensor([0.999, 0.001])
