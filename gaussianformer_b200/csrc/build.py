@@ -27,7 +27,7 @@ def _stale() -> bool:
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(HERE, f) for f in SOURCES + ["common.cuh", "splat_render.cuh", "splat_tile.cuh", "splat_bwd_common.cuh", "daf_pair.cuh"]] + [os.path.join(ROOT, "include", "gf_b200.h"), os.path.join(ROOT, "include", "gf_b200_debug.h")]
+    deps = [os.path.join(HERE, f) for f in SOURCES + ["common.cuh", "splat_render.cuh", "splat_tile.cuh", "splat_bwd_common.cuh", "splat_host.cuh", "daf_pair.cuh"]] + [os.path.join(ROOT, "include", "gf_b200.h"), os.path.join(ROOT, "include", "gf_b200_debug.h")]
     return any(os.path.getmtime(d) > t for d in deps)
 
 

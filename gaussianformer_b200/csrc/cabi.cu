@@ -7,6 +7,7 @@
 #include "common.cuh"
 #include "daf_pair.cuh"
 #include "gf_b200_debug.h"
+#include "splat_host.cuh"
 
 namespace gf {
 
@@ -23,23 +24,6 @@ int cuda_fail(cudaError_t e, const char *what) {
     set_error("CUDA error %d (%s) in %s", static_cast<int>(e), cudaGetErrorString(e), what);
     return GF_ERR_CUDA;
 }
-
-// defined in the kernel translation units
-int plan_forward_workspace(const gf_splat_desc &d, void *base, SplatWorkspace *ws);
-int launch_prep(const gf_splat_desc &d, const gf_splat_inputs &in, const SplatWorkspace &ws, uint32_t initial_flags,
-                cudaStream_t stream, bool raw_records = false);
-int launch_render(const gf_splat_desc &d, const gf_splat_inputs &in, const gf_splat_outputs &out,
-                  const SplatWorkspace &ws, bool tile_path, int num_sms, cudaStream_t stream);
-size_t backward_workspace_bytes(const gf_splat_desc &d);
-int launch_backward(const gf_splat_desc &d, const gf_splat_inputs &in, const gf_splat_grads &gr, void *workspace,
-                    int num_sms, cudaStream_t stream);
-int render_ctas_per_sample(const gf_splat_desc &d);
-extern thread_local cudaEvent_t g_ev_before, g_ev_after;
-
-int launch_daf(const DafParams &p, bool backward, int num_sms, cudaStream_t stream);
-int launch_daf_format(const gf_daf_format_desc &d, float *const *maps, float *table, bool inverse, cudaStream_t stream);
-bool daf_fused_supported(const gf_daf_desc &d, int K);
-int launch_daf_fused(const DafFusedParams &p, bool backward, int num_sms, cudaStream_t stream);
 
 thread_local cudaEvent_t g_ev_before = nullptr, g_ev_after = nullptr;
 
@@ -114,9 +98,9 @@ int gf_splat_supported_classes(int32_t *out, int cap) {
 
 size_t gf_splat_forward_workspace_bytes(const gf_splat_desc *desc) {
     if (check_desc(desc) != GF_OK) return 0;
-    SplatWorkspace ws;
-    plan_forward_workspace(*desc, nullptr, &ws);
-    return ws.bytes;
+    WorkspaceCarver carve{nullptr};
+    plan_forward_workspace(*desc, carve);
+    return carve.bytes;
 }
 
 int gf_splat_ce_partials(const gf_splat_desc *desc) {
@@ -145,10 +129,10 @@ int gf_splat_forward(const gf_splat_desc *desc, const gf_splat_inputs *in, const
     if (desc->variant == GF_SPLAT_PROB && desc->N > 0)
         GF_REQUIRE(out->bin_logits && out->density && out->probability, GF_ERR_INVALID_ARG,
                    "splat(prob): bin_logits / density / probability must not be NULL");
-    SplatWorkspace ws;
-    plan_forward_workspace(*desc, workspace, &ws);
-    GF_REQUIRE(workspace != nullptr && workspace_bytes >= ws.bytes, GF_ERR_WORKSPACE,
-               "splat: workspace too small (%zu < %zu bytes)", workspace_bytes, ws.bytes);
+    WorkspaceCarver carve{static_cast<char *>(workspace)};
+    const SplatWorkspace ws = plan_forward_workspace(*desc, carve);
+    GF_REQUIRE(workspace != nullptr && workspace_bytes >= carve.bytes, GF_ERR_WORKSPACE,
+               "splat: workspace too small (%zu < %zu bytes)", workspace_bytes, carve.bytes);
     GF_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255u) == 0, GF_ERR_WORKSPACE,
                "splat: workspace must be 256-byte aligned");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);

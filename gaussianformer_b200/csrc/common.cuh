@@ -51,9 +51,6 @@ constexpr int kBinX = 8;        // render CTA footprint in columns: 8 (x) by 4 (
 constexpr int kBinY = 4;
 constexpr int kBinZ = 16;       // ... by 16 voxels in z (one z-chunk)
 constexpr int kRenderThreads = 128;
-constexpr int kVox = 4;         // voxels per thread (a z-quad)
-constexpr int kChunk = 32;      // Gaussian records staged per TMA batch
-constexpr int kSeg = 512;       // bin-list entries resolved per segment
 constexpr int kGeomFloats = 12; // mu(3) k(1) c6(6) pad(2)
 
 __host__ __device__ constexpr int round_up(int v, int m) { return (v + m - 1) / m * m; }
@@ -70,21 +67,23 @@ struct __align__(16) PackedBox {
     uint32_t x, y, z, empty;
 };
 
+// The forward workspace of the splat pipeline (also the forward-style block of the backward workspace).  Only
+// plan_forward_workspace (splat_prep.cu) decides its layout; kernels receive it whole and narrow it to one sample with
+// sample_ws and number supertiles with supertile_of.
 struct SplatWorkspace {
-    // all pointers carved out of the caller's workspace by carve_forward_workspace()
-    uint32_t *flags;       // [16]  status word(s)
-    uint32_t *pack_flags;  // [pack_ctas] per-CTA error bits of the pack kernel
-    float *records;        // [G, rec_floats(C)]
-    PackedBox *boxes;      // [G]
-    uint32_t *masks;       // [nsuper, nwords] bit g of supertile s: box(g) overlaps s
-    int32_t *lists;        // [nsuper, G] ascending Gaussian indices per supertile
-    int32_t *counts;       // [nsuper]
-    int st;                // supertile edge (columns)
+    uint32_t *flags;       // status block, 256 bytes: word 0 status bits, words 4..19 GF_RENDER_TIMING cycle counters
+    uint32_t *pack_flags;  // [batch * pack_ctas] per-CTA error bits of the pack kernel
+    float *records;        // [G, rec] per sample
+    PackedBox *boxes;      // [G] per sample
+    uint32_t *masks;       // [nsuper, nwords] per sample: bit g of supertile s: box(g) overlaps s
+    int32_t *lists;        // [nsuper, G] per sample: ascending Gaussian indices per supertile
+    int32_t *counts;       // [nsuper] per sample
+    int rec;               // floats per record: rec_floats(C)
+    int st;                // supertile edge (columns), a power of two
     int nsx, nsy, nsuper;  // supertile grid
     int nwords;            // ceil(G/32)
     int pack_ctas;         // pack CTAs per sample
-    int batch;             // samples; every region above except `flags` holds `batch` consecutive per-sample blocks
-    size_t bytes;
+    int batch;             // samples
 };
 
 __host__ __device__ inline int batch_of(const gf_splat_desc &d) { return d.batch > 0 ? d.batch : 1; }
@@ -162,16 +161,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
         if (++spins > (1u << 24)) __trap();
     }
 }
-// 1-D bulk async copy global -> shared through the TMA unit, completion counted on an mbarrier.
-__device__ __forceinline__ void tma_load_1d(void *smem_dst, const void *gmem_src, uint32_t bytes,
-                                            uint64_t *bar) {
-    asm volatile(
-        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-            smem_u32(smem_dst)),
-        "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
-        : "memory");
-}
-
 // Programmatic dependent launch (the three kernels of a forward call are chained with it, see
 // launch_chained): launch_dependents lets the next kernel of the stream become resident while this grid
 // is still running; wait blocks until the preceding grid has completed and its writes are visible.
@@ -188,16 +177,16 @@ __device__ __forceinline__ uint32_t lanemask_lt() {
 // Phase A of the bin kernels (render_tile_kernel, backward_bin_kernel): the bin's ordered Gaussian list, resolved from
 // its supertile's list.  A bin entry is one Gaussian whose box overlaps the bin: .x holds the box clipped to the bin as
 // bit masks -- x columns in bits 0-7, y columns in bits 8-11, z levels in bits 16-31 -- and .y the Gaussian index.
-// All NT threads of the CTA test the candidates cand[cpos..ncand), the ascending list of supertile s (`lists`: [nsuper,
-// G]), fetching kPre rounds of NT before testing any (memory-level parallelism), and append the survivors to `list` in
-// the same order, compacted with ballots, until the candidates run out or another round might overflow SEG entries.
-// Advances cpos past the tested candidates and returns the number of entries.
+// All NT threads of the CTA test the candidates cand[cpos..ncand), the ascending list of supertile s of the sample `ws`
+// is narrowed to, fetching kPre rounds of NT before testing any (memory-level parallelism), and append the survivors to
+// `list` in the same order, compacted with ballots, until the candidates run out or another round might overflow SEG
+// entries.  Advances cpos past the tested candidates and returns the number of entries.
 template <int NT, int kPre, int SEG>
-__device__ __forceinline__ int resolve_bin_list(const gf_splat_desc &d, const int32_t *lists, int s, int ncand, int &cpos,
-                                                const PackedBox *boxes, int binX0, int binY0, int binZ0, uint2 *list,
-                                                int (&warp_count)[2][NT / 32]) {
+__device__ __forceinline__ int resolve_bin_list(const gf_splat_desc &d, const SplatWorkspace &ws, int s, int ncand, int &cpos,
+                                                int binX0, int binY0, int binZ0, uint2 *list, int (&warp_count)[2][NT / 32]) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int32_t *cand = lists + static_cast<size_t>(s) * d.G;
+    const int32_t *cand = ws.lists + static_cast<size_t>(s) * d.G;
+    const PackedBox *boxes = ws.boxes;
     const uint32_t bX1 = min(binX0 + kBinX, d.H) - 1, bY1 = min(binY0 + kBinY, d.W) - 1, bZ1 = min(binZ0 + kBinZ, d.D) - 1;
     int nlist = 0;
     while (cpos < ncand && nlist + NT <= SEG) {
@@ -317,6 +306,23 @@ __device__ __forceinline__ gf_splat_inputs sample_inputs(const gf_splat_desc &d,
     return o;
 }
 
+// The workspace blocks of sample b: records, boxes, masks, lists and counts.  flags and pack_flags stay batch-level.
+__device__ __forceinline__ SplatWorkspace sample_ws(const SplatWorkspace &ws, int G, int b) {
+    SplatWorkspace o = ws;
+    o.records = ws.records + static_cast<size_t>(b) * G * ws.rec;
+    o.boxes = ws.boxes + static_cast<size_t>(b) * G;
+    o.masks = ws.masks + static_cast<size_t>(b) * ws.nsuper * ws.nwords;
+    o.lists = ws.lists + static_cast<size_t>(b) * ws.nsuper * G;
+    o.counts = ws.counts + static_cast<size_t>(b) * ws.nsuper;
+    return o;
+}
+
+// Supertile of column (x, y) (x, y >= 0): supertiles are st x st columns, numbered x-major.
+__device__ __forceinline__ int supertile_of(const SplatWorkspace &ws, int x, int y) {
+    const int sh = 31 - __clz(ws.st);
+    return (x >> sh) * ws.nsy + (y >> sh);
+}
+
 __device__ __forceinline__ gf_splat_outputs sample_outputs(const gf_splat_desc &d, const gf_splat_outputs &out, int b, int ce_rows) {
     gf_splat_outputs o;
     const long long N = d.N;
@@ -386,17 +392,6 @@ __device__ __forceinline__ void load_cov6_in(const gf_splat_desc &d, const gf_sp
     } else {
 #pragma unroll
         for (int i = 0; i < 6; ++i) c6[i] = __ldg(cv + i);
-    }
-}
-
-// the six inverse-covariance entries (xx,yy,zz,xy,yz,xz) of Gaussian g
-__device__ __forceinline__ void load_cov6(const gf_splat_desc &d, const float *cov, int g, float c6[6]) {
-    const float *cv = cov + static_cast<size_t>(g) * d.cov_stride;
-    if (d.cov_stride == 9) {  // flat entries [0,4,8,1,5,2] of the row-major 3x3 (__init__.py:143)
-        c6[0] = cv[0]; c6[1] = cv[4]; c6[2] = cv[8]; c6[3] = cv[1]; c6[4] = cv[5]; c6[5] = cv[2];
-    } else {
-#pragma unroll
-        for (int i = 0; i < 6; ++i) c6[i] = cv[i];
     }
 }
 

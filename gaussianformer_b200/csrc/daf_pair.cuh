@@ -45,6 +45,13 @@ struct DafFusedParams {
     float *grad_feat, *grad_loc, *grad_logits;
 };
 
+// daf.cu
+int launch_daf(const DafParams &p, bool backward, int num_sms, cudaStream_t stream);
+int launch_daf_format(const gf_daf_format_desc &d, float *const *maps, float *table, bool inverse, cudaStream_t stream);
+// daf_fused.cu
+bool daf_fused_supported(const gf_daf_desc &d, int K);
+int launch_daf_fused(const DafFusedParams &p, bool backward, int num_sms, cudaStream_t stream);
+
 struct PairSetup {     // 64 bytes per (camera, level) pair
     int row[4];        // element offset of each corner row inside the batch's feature block (row * C)
     float w[4];        // bilinear corner weights, 0 where the corner is outside the map

@@ -17,6 +17,7 @@
 //                         of small queued boxes is walked Gaussian by Gaussian); block reduction +
 //                         one atomicAdd per scalar and (CTA, Gaussian) segment.
 #include "splat_bwd_common.cuh"
+#include "splat_host.cuh"
 
 namespace gf {
 
@@ -249,20 +250,13 @@ __global__ void __launch_bounds__(128) srt_grad_kernel(const BwdParams pb) {
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-int plan_forward_workspace(const gf_splat_desc &d, void *base, SplatWorkspace *ws);   // splat_prep.cu
-int launch_prep(const gf_splat_desc &d, const gf_splat_inputs &in, const SplatWorkspace &ws, uint32_t initial_flags,
-                cudaStream_t stream, bool raw_records = false);
-bool backward_bin_eligible(const gf_splat_desc &d, const gf_splat_inputs &in, const gf_splat_grads &gr);   // splat_backward_bin.cu
-int launch_backward_bin(const BwdParams &bp, const SplatWorkspace &fws, float *sums, cudaStream_t stream);
-
 struct BwdWorkspace {
     int32_t *v2p, *canon;
     unsigned long long *big_ctr;
     uint2 *big;
     float4 *aux;
     float *cov6;       // [B,G,6] gradient of Sigma^-1 when the caller passed scales + rotations instead of cov
-    void *fwd;         // boxes + supertile lists for the bin-centric kernel (a forward-style workspace; 256-byte aligned)
-    size_t fwd_bytes;
+    SplatWorkspace fwd;   // records, boxes and supertile lists for the bin-centric kernel
     float *sums;       // [B,G,32] raw sums of the bin-centric kernel
     size_t sums_bytes;
     size_t cv_block;   // bytes of one sample's (canon word, voxel -> point map) block
@@ -279,33 +273,22 @@ static int chunk_voxels(const gf_splat_desc &d) {
     return static_cast<int>(c);
 }
 
-static size_t align_up_b(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
 void plan_backward_workspace(const gf_splat_desc &d, void *base, BwdWorkspace *ws) {
-    size_t off = 0;
-    char *b = static_cast<char *>(base);
+    WorkspaceCarver carve{static_cast<char *>(base)};
     const size_t B = static_cast<size_t>(batch_of(d));
-    auto take = [&](size_t bytes) {
-        char *p = b ? b + off : nullptr;
-        off = align_up_b(off + bytes, 256);
-        return p;
-    };
-    ws->big_ctr = reinterpret_cast<unsigned long long *>(take(B * 8));
+    ws->big_ctr = carve.take<unsigned long long>(B * 8);
     // per sample: the canon word (256 bytes) directly in front of its voxel -> point map; one memset covers all
-    ws->cv_block = 256 + align_up_b(size_t(d.H) * d.W * d.D * 4, 256);
+    ws->cv_block = 256 + WorkspaceCarver::align(size_t(d.H) * d.W * d.D * 4);
     ws->cv_bytes = B * ws->cv_block;
-    ws->canon = reinterpret_cast<int32_t *>(take(ws->cv_bytes));
+    ws->canon = carve.take<int32_t>(ws->cv_bytes);
     ws->v2p = ws->canon ? ws->canon + 64 : nullptr;
-    ws->big = reinterpret_cast<uint2 *>(take(B * size_t(d.G) * sizeof(uint2)));
-    ws->aux = reinterpret_cast<float4 *>(take(d.variant == GF_SPLAT_PROB ? B * size_t(d.N) * 16 : 0));
-    ws->cov6 = reinterpret_cast<float *>(take(B * size_t(d.G) * 6 * 4));   // only used with scales + rotations input
-    SplatWorkspace fws;
-    plan_forward_workspace(d, nullptr, &fws);
-    ws->fwd_bytes = fws.bytes;
-    ws->fwd = take(fws.bytes);
+    ws->big = carve.take<uint2>(B * size_t(d.G) * sizeof(uint2));
+    ws->aux = carve.take<float4>(d.variant == GF_SPLAT_PROB ? B * size_t(d.N) * 16 : 0);
+    ws->cov6 = carve.take<float>(B * size_t(d.G) * 6 * 4);   // only used with scales + rotations input
+    ws->fwd = plan_forward_workspace(d, carve);
     ws->sums_bytes = B * size_t(d.G) * 32 * 4;
-    ws->sums = reinterpret_cast<float *>(take(ws->sums_bytes));
-    ws->bytes = off;
+    ws->sums = carve.take<float>(ws->sums_bytes);
+    ws->bytes = carve.bytes;
 }
 
 size_t backward_workspace_bytes(const gf_splat_desc &d) {
@@ -332,11 +315,9 @@ static int launch_backward_t(const BwdParams &bp, const BwdWorkspace &ws, bool s
             prob_aux_kernel<<<dim3(grid0, B), 256, 0, stream>>>(bp, C);
             GF_CUDA_TRY(cudaGetLastError());
         }
-        SplatWorkspace fws;
-        plan_forward_workspace(d, ws.fwd, &fws);
-        int rc = launch_prep(d, bp.in, fws, 0u, stream, true);
+        int rc = launch_prep(d, bp.in, ws.fwd, 0u, stream, true);
         if (rc != GF_OK) return rc;
-        rc = launch_backward_bin(bp, fws, ws.sums, stream);
+        rc = launch_backward_bin(bp, ws.fwd, ws.sums, stream);
         if (rc != GF_OK) return rc;
         // the Gaussian-centric chain is only the fallback now: small grids (they return at once when the points are canonical)
         GF_CUDA_TRY(launch_chained(voxel_map_kernel, dim3(num_sms, B), dim3(256), 0, stream, bp));

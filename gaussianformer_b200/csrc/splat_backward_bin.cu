@@ -26,6 +26,7 @@
 #include <cuda.h>
 
 #include "splat_bwd_common.cuh"
+#include "splat_host.cuh"
 
 namespace gf {
 
@@ -45,12 +46,8 @@ struct alignas(64) BinMaps {
 };
 
 struct BinParams {
-    const float *records;     // raw records of the pack kernel: [B*G, 32]
+    SplatWorkspace ws;        // raw records of the pack kernel, boxes and supertile lists
     float *sums;              // [B, 32, G] raw sums (value-major), zero-filled by the host
-    const PackedBox *boxes;
-    const int32_t *lists;
-    const int32_t *counts;
-    int st, nsy, nsuper;
     int nbx;
 };
 
@@ -158,10 +155,9 @@ __global__ void __launch_bounds__(kBinThreads, 2) backward_bin_kernel(const BwdP
     }
 
     // ---- candidates: the ascending list of this bin's supertile ------------------------------------------------
-    const int st_shift = 31 - __clz(bp.st);
-    const int s = sample * bp.nsuper + (binX0 >> st_shift) * bp.nsy + (binY0 >> st_shift);
-    const int ncand = bp.counts[s];
-    const PackedBox *boxes = bp.boxes + static_cast<size_t>(sample) * p.d.G;
+    const SplatWorkspace ws = sample_ws(bp.ws, p.d.G, sample);
+    const int s = supertile_of(ws, binX0, binY0);
+    const int ncand = ws.counts[s];
     if (ncand == 0) {
         // No Gaussian to walk, but the point order is still this bin's to check: a point stored here may lie in a
         // covered voxel (several points in one voxel).  Waiting also keeps the CTA from exiting with its copies in flight.
@@ -176,8 +172,7 @@ __global__ void __launch_bounds__(kBinThreads, 2) backward_bin_kernel(const BwdP
         if (tid == 0) sm.next = 0;   // published by the barriers of Phase A
         if (tid <= kVolKeys) sm.hist[tid] = 0;
         // ======================= Phase A: ordered survivors of the box test ==========================
-        const int nlist = resolve_bin_list<NT, 2, kBinSeg>(p.d, bp.lists, s, ncand, cpos, boxes, binX0, binY0, binZ0, sm.list,
-                                                           sm.warp_count);
+        const int nlist = resolve_bin_list<NT, 2, kBinSeg>(p.d, ws, s, ncand, cpos, binX0, binY0, binZ0, sm.list, sm.warp_count);
         // ---- order the entries by clipped-box volume (counting sort; the order of the sum does not matter here) ----
         int mykey[kBinSeg / NT];
 #pragma unroll
@@ -221,7 +216,6 @@ __global__ void __launch_bounds__(kBinThreads, 2) backward_bin_kernel(const BwdP
         __syncthreads();
 
         // ======================= Phase B: eight lanes (or a whole warp) per listed Gaussian ===========
-        const float *records = bp.records + static_cast<size_t>(sample) * p.d.G * 32;
         float *sums = bp.sums + static_cast<size_t>(sample) * p.d.G * 32;
         const int n_narrow = sm.n_narrow, narrow_tickets = (n_narrow + 3) >> 2;
         const int tickets = narrow_tickets + (nlist - n_narrow);
@@ -241,7 +235,7 @@ __global__ void __launch_bounds__(kBinThreads, 2) backward_bin_kernel(const BwdP
             const int x0 = __ffs(xm) - 1, nx = __popc(xm), y0 = __ffs(ym) - 1, ny = __popc(ym), z0 = __ffs(zm) - 1, nz = __popc(zm);
             const int vol = nx * ny * nz;   // 0 for a lane group without an entry
             GaussAcc<C, PROB> acc;
-            acc.load_record(reinterpret_cast<const float4 *>(records + static_cast<size_t>(g) * 32));
+            acc.load_record(reinterpret_cast<const float4 *>(ws.records + static_cast<size_t>(g) * rec_floats(C)));
             // My lanes stride over the clipped box, z fastest; the stride is decomposed once into box steps.  A whole-warp
             // entry walks the two z halves of the box one after the other: the halves of the gradient tile are two TMA
             // boxes whose distance is a multiple of 128 bytes, so lanes on the same column and z & 7 of different halves
@@ -425,16 +419,7 @@ int launch_backward_bin(const BwdParams &bp, const SplatWorkspace &fws, float *s
     if (d.variant == GF_SPLAT_PROB) ok = ok && make_map(&maps.aux, bp.aux, B * d.H, d.W, d.D * 4, kBinZ * 4);
     else maps.aux = maps.pts;
     GF_REQUIRE(ok, GF_ERR_CUDA, "splat backward: cuTensorMapEncodeTiled failed");
-    BinParams np;
-    np.records = fws.records;
-    np.sums = sums;
-    np.boxes = fws.boxes;
-    np.lists = fws.lists;
-    np.counts = fws.counts;
-    np.st = fws.st;
-    np.nsy = fws.nsy;
-    np.nsuper = fws.nsuper;
-    np.nbx = (d.H + kBinX - 1) / kBinX;
+    const BinParams np{fws, sums, (d.H + kBinX - 1) / kBinX};
     const bool prob = d.variant == GF_SPLAT_PROB;
     return dispatch_classes(d.C, "splat backward", [&](auto cc) {
         constexpr int C = decltype(cc)::value;

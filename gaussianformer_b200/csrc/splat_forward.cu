@@ -5,11 +5,10 @@
 //                       comment below); stray points are detected per voxel and re-evaluated exactly.
 // render_points_kernel  arbitrary points (N != H*W*D, several per voxel): one thread per point walks
 //                       the supertile list with the exact box test.
+#include "splat_host.cuh"
 #include "splat_tile.cuh"
 
 namespace gf {
-
-extern thread_local cudaEvent_t g_ev_before, g_ev_after;  // measurement hooks (cabi.cu)
 
 // SIMT render kernel: bin = 8 x 4 columns x 16 z, 4 consecutive z voxels per thread with 4 x C accumulators in
 // registers (36 packed fp32 pairs); a warp covers 4 x 4 columns x 8 z.  128 threads, 128 registers, 4 CTAs per SM.
@@ -123,7 +122,7 @@ __global__ void __launch_bounds__(kRenderThreads, PROB ? 3 : 4) render_tile_kern
     // Everything above depends on the caller's inputs only; the records, boxes, lists and the status word
     // come from the two preparation kernels, which this grid may have been launched ahead of.
     pdl_wait();
-    if (stray) atomicOr(pin.flags, GF_FLAG_GENERIC_PATH);
+    if (stray) atomicOr(pin.ws.flags, GF_FLAG_GENERIC_PATH);
 #ifdef GF_RENDER_TIMING
     if (tid == 0) sm.t_phase[0] = static_cast<unsigned long long>(clock64() - t_start);
 #endif
@@ -346,7 +345,7 @@ __global__ void __launch_bounds__(kRenderThreads, PROB ? 3 : 4) render_tile_kern
     }
 #ifdef GF_RENDER_TIMING
     if (tid == 0) {
-        unsigned long long *t = reinterpret_cast<unsigned long long *>(p.flags + 4);   // bytes 16..47 of the status block
+        unsigned long long *t = reinterpret_cast<unsigned long long *>(p.ws.flags + 4);   // bytes 16..47 of the status block
         atomicAdd(t + 0, sm.t_phase[0]);
         atomicAdd(t + 1, sm.t_phase[1]);
         atomicAdd(t + 2, sm.t_phase[2]);
@@ -359,9 +358,10 @@ __global__ void __launch_bounds__(kRenderThreads, PROB ? 3 : 4) render_tile_kern
 // ------------------------------------------------------------------------------------------------
 // generic path: arbitrary points
 // ------------------------------------------------------------------------------------------------
+// Launched only when N != H*W*D, the case for which gf_splat_forward seeds the status word with GF_FLAG_GENERIC_PATH
+// (written by list_kernel), so the flag needs no check here.
 template <int C, bool PROB>
 __global__ void __launch_bounds__(256) render_points_kernel(const RenderParams pb) {
-    if (!(*reinterpret_cast<volatile uint32_t *>(pb.flags) & GF_FLAG_GENERIC_PATH)) return;
     const RenderParams p = with_sample_outputs(sample_params(pb, blockIdx.y), pb, blockIdx.y);
     for (long long n = blockIdx.x * 256ll + threadIdx.x; n < p.d.N; n += 256ll * gridDim.x)
         render_one_point<C, PROB>(p, n, p.pts[3 * n], p.pts[3 * n + 1], p.pts[3 * n + 2]);
@@ -407,17 +407,10 @@ int launch_render(const gf_splat_desc &d, const gf_splat_inputs &in, const gf_sp
     rp.pts = in.pts;
     rp.points_int = in.points_int;
     rp.out = out;
-    rp.records = ws.records;
-    rp.boxes = ws.boxes;
-    rp.lists = ws.lists;
-    rp.counts = ws.counts;
-    rp.flags = ws.flags;
-    rp.st = ws.st;
-    rp.nsy = ws.nsy;
+    rp.ws = ws;
     rp.nby = (d.W + kBinY - 1) / kBinY;
     rp.nzc = (d.D + kBinZ - 1) / kBinZ;
     rp.nbx = (d.H + kBinX - 1) / kBinX;
-    rp.nsuper = ws.nsuper;
     rp.ce_rows = render_ctas_per_sample(d);
     // 16-byte vector accesses need D % 4 == 0 (a thread's z quad is then 4 consecutive points of every tensor) and
     // 16-byte aligned tensors; anything else takes the scalar loads / stores of the same kernel

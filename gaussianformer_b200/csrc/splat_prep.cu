@@ -11,22 +11,15 @@
 //                      integer box, and one ballot bit per supertile (16x16 columns) it overlaps.
 //   list_kernel        one CTA per supertile: popcount-scan of the mask words -> ascending
 //                      Gaussian index list (ascending order == the reference's stable sort order).
-#include "common.cuh"
+#include "splat_host.cuh"
 
 namespace gf {
 
 struct PackParams {
     gf_splat_desc d;
     gf_splat_inputs in;
-    float *records;
-    PackedBox *boxes;
-    uint32_t *masks;
-    uint32_t *pack_flags;
-    int rec;     // floats per record
+    SplatWorkspace ws;
     int raw;     // != 0: records for the bin-centric backward -- (mu, opacity | c6 as given | sem as given), nothing folded
-    int st;      // supertile edge
-    int nsx, nsy;
-    int nwords;
 };
 
 constexpr int kMaskPass = 1024;  // supertiles resolved per shared-memory pass
@@ -37,12 +30,11 @@ __global__ void __launch_bounds__(kPackThreads) pack_mask_kernel(const PackParam
     const int g = blockIdx.x * kPackThreads + threadIdx.x;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const bool live = g < p.d.G;
-    // sample b of the batch: its input tensors and its blocks of the workspace regions
+    // sample b of the batch: its input tensors and its blocks of the workspace regions (the region sizes are the same
+    // for every sample and are read from p.ws)
     const int b = blockIdx.y;
     const gf_splat_inputs in = sample_inputs(p.d, p.in, b);
-    float *const records = p.records + static_cast<size_t>(b) * p.d.G * p.rec;
-    PackedBox *const boxes = p.boxes + static_cast<size_t>(b) * p.d.G;
-    uint32_t *const masks = p.masks + static_cast<size_t>(b) * p.nsx * p.nsy * p.nwords;
+    const SplatWorkspace ws = sample_ws(p.ws, p.d.G, b);
     if (threadIdx.x == 0) s_err = 0;
     pdl_launch_dependents();   // the list kernel may become resident now; it waits for this grid before reading
 
@@ -55,7 +47,7 @@ __global__ void __launch_bounds__(kPackThreads) pack_mask_kernel(const PackParam
         float c6[6];
         load_cov6_in(p.d, in, g, c6);   // the caller's Sigma^-1, or R^T diag(1/s^2) R from scales + rotations (cov == NULL)
         float amp = __ldg(in.opacities + g);
-        const int nq = (p.rec - kGeomFloats) / 4;   // <= 5 for C <= 20
+        const int nq = (p.ws.rec - kGeomFloats) / 4;   // <= 5 for C <= 20
         float semv[20];
         {
             const float *sem = in.semantics + static_cast<size_t>(g) * p.d.C;
@@ -69,7 +61,7 @@ __global__ void __launch_bounds__(kPackThreads) pack_mask_kernel(const PackParam
         bx.y = empty ? 1u : (static_cast<uint32_t>(lo[1]) | static_cast<uint32_t>(hi[1]) << 16);
         bx.z = empty ? 1u : (static_cast<uint32_t>(lo[2]) | static_cast<uint32_t>(hi[2]) << 16);
         bx.empty = empty ? 1u : 0u;
-        boxes[g] = bx;
+        ws.boxes[g] = bx;
 
         const float a_ = c6[0], b_ = c6[1], c_ = c6[2], d_ = c6[3], e_ = c6[4], f_ = c6[5];
         if (p.raw) {
@@ -90,7 +82,7 @@ __global__ void __launch_bounds__(kPackThreads) pack_mask_kernel(const PackParam
             if (!empty && p.d.D <= 32) zmask = ((2u << hi[2]) - 1u) & ~((1u << lo[2]) - 1u);
             amp = __uint_as_float(zmask);
         }
-        float4 *rec = reinterpret_cast<float4 *>(records + static_cast<size_t>(g) * p.rec);
+        float4 *rec = reinterpret_cast<float4 *>(ws.records + static_cast<size_t>(g) * p.ws.rec);
         rec[0] = make_float4(mu[0], mu[1], mu[2], amp);
         if (p.raw) {
             rec[1] = make_float4(a_, b_, c_, d_);
@@ -108,11 +100,11 @@ __global__ void __launch_bounds__(kPackThreads) pack_mask_kernel(const PackParam
     }
 
     // ---- supertile masks: per-warp words assembled in shared memory, stored by all lanes ------------
-    const int sx0 = empty ? 1 : lo[0] / p.st, sx1 = empty ? 0 : hi[0] / p.st;
-    const int sy0 = empty ? 1 : lo[1] / p.st, sy1 = empty ? 0 : hi[1] / p.st;
+    const int sx0 = empty ? 1 : lo[0] / p.ws.st, sx1 = empty ? 0 : hi[0] / p.ws.st;
+    const int sy0 = empty ? 1 : lo[1] / p.ws.st, sy1 = empty ? 0 : hi[1] / p.ws.st;
     const int word = g >> 5;          // warp-uniform
-    const int nsuper = p.nsx * p.nsy;
-    if (word < p.nwords) {
+    const int nsuper = p.ws.nsuper;
+    if (word < p.ws.nwords) {
         for (int base = 0; base < nsuper; base += kMaskPass) {
             const int npass = min(kMaskPass, nsuper - base);
             for (int i = lane; i < npass; i += 32) s_mask[warp][i] = 0u;
@@ -121,10 +113,10 @@ __global__ void __launch_bounds__(kPackThreads) pack_mask_kernel(const PackParam
             // whole-grid "empty" Gaussian touches all of them) is spread over the 32 lanes instead
             const int ny = sy1 - sy0 + 1, cnt = empty ? 0 : (sx1 - sx0 + 1) * ny;
             const bool wide = cnt > 16;
-            if (!wide)
-                for (int sx = sx0; sx <= sx1; ++sx)
-                    for (int sy = sy0; sy <= sy1; ++sy) {
-                        const int s = sx * p.nsy + sy - base;
+            if (!wide)   // a column of each supertile the box touches
+                for (int x = sx0 * p.ws.st; x <= sx1 * p.ws.st; x += p.ws.st)
+                    for (int y = sy0 * p.ws.st; y <= sy1 * p.ws.st; y += p.ws.st) {
+                        const int s = supertile_of(p.ws, x, y) - base;
                         if (s >= 0 && s < npass) atomicOr(&s_mask[warp][s], 1u << lane);
                     }
             uint32_t wides = __ballot_sync(0xffffffffu, wide);
@@ -134,13 +126,13 @@ __global__ void __launch_bounds__(kPackThreads) pack_mask_kernel(const PackParam
                 const int wx0 = __shfl_sync(0xffffffffu, sx0, src), wy0 = __shfl_sync(0xffffffffu, sy0, src);
                 const int wny = __shfl_sync(0xffffffffu, ny, src), wcnt = __shfl_sync(0xffffffffu, cnt, src);
                 for (int i = lane; i < wcnt; i += 32) {
-                    const int s = (wx0 + i / wny) * p.nsy + (wy0 + i % wny) - base;
+                    const int s = supertile_of(p.ws, (wx0 + i / wny) * p.ws.st, (wy0 + i % wny) * p.ws.st) - base;
                     if (s >= 0 && s < npass) atomicOr(&s_mask[warp][s], 1u << src);
                 }
             }
             __syncwarp();
             for (int i = lane; i < npass; i += 32)
-                masks[static_cast<size_t>(base + i) * p.nwords + word] = s_mask[warp][i];
+                ws.masks[static_cast<size_t>(base + i) * p.ws.nwords + word] = s_mask[warp][i];
             __syncwarp();
         }
     }
@@ -149,18 +141,12 @@ __global__ void __launch_bounds__(kPackThreads) pack_mask_kernel(const PackParam
     __syncthreads();
     if (err) atomicOr(&s_err, err);
     __syncthreads();
-    if (threadIdx.x == 0) p.pack_flags[blockIdx.y * gridDim.x + blockIdx.x] = s_err;
+    if (threadIdx.x == 0) p.ws.pack_flags[blockIdx.y * gridDim.x + blockIdx.x] = s_err;
 }
 
 struct ListParams {
-    const uint32_t *masks;
-    const uint32_t *pack_flags;
-    int32_t *lists;
-    int32_t *counts;
-    uint32_t *flags;
-    int nwords;
+    SplatWorkspace ws;
     int G;
-    int pack_ctas;   // pack CTAs of the whole batch
     uint32_t initial_flags;
 };
 
@@ -168,21 +154,22 @@ constexpr int kListThreads = 256;
 constexpr int kListWordsPerThread = 4;   // consecutive mask words per thread and pass (keeps ascending order)
 
 __global__ void __launch_bounds__(kListThreads) list_kernel(const ListParams p) {
-    const int s = blockIdx.y * gridDim.x + blockIdx.x;   // supertile blockIdx.x of sample blockIdx.y
-    const uint32_t *words = p.masks + static_cast<size_t>(s) * p.nwords;
-    int32_t *list = p.lists + static_cast<size_t>(s) * p.G;
+    const SplatWorkspace ws = sample_ws(p.ws, p.G, blockIdx.y);
+    const int s = blockIdx.x;   // supertile s of sample blockIdx.y
+    const uint32_t *words = ws.masks + static_cast<size_t>(s) * ws.nwords;
+    int32_t *list = ws.lists + static_cast<size_t>(s) * p.G;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     __shared__ int s_warp[2][kListThreads / 32];
     pdl_launch_dependents();   // lets the render kernel start its point prologue
     pdl_wait();                // masks and flags of the pack kernel are complete from here on
     int base = 0, pass = 0;
-    for (int w0 = 0; w0 < p.nwords; w0 += kListThreads * kListWordsPerThread, ++pass) {
+    for (int w0 = 0; w0 < ws.nwords; w0 += kListThreads * kListWordsPerThread, ++pass) {
         const int first = w0 + threadIdx.x * kListWordsPerThread;
         uint32_t bits[kListWordsPerThread];
         int cnt = 0;
 #pragma unroll
         for (int i = 0; i < kListWordsPerThread; ++i) {
-            bits[i] = first + i < p.nwords ? __ldg(words + first + i) : 0u;
+            bits[i] = first + i < ws.nwords ? __ldg(words + first + i) : 0u;
             cnt += __popc(bits[i]);
         }
         int incl = cnt;  // inclusive warp scan
@@ -212,28 +199,27 @@ __global__ void __launch_bounds__(kListThreads) list_kernel(const ListParams p) 
         }
         base += total;
     }
-    if (threadIdx.x == 0) p.counts[s] = base;
+    if (threadIdx.x == 0) ws.counts[s] = base;
 
-    if (s == 0) {  // fold the pack kernel's error bits into the status word (also initialises it)
+    if (s == 0 && blockIdx.y == 0) {  // fold the pack kernel's error bits into the status word (also initialises it)
         uint32_t e = 0;
-        for (int i = threadIdx.x; i < p.pack_ctas; i += kListThreads) e |= p.pack_flags[i];
+        for (int i = threadIdx.x; i < ws.pack_ctas * ws.batch; i += kListThreads) e |= ws.pack_flags[i];
         e = __reduce_or_sync(0xffffffffu, e);
         __shared__ uint32_t s_e;
         if (threadIdx.x == 0) s_e = p.initial_flags;
         __syncthreads();
         if (lane == 0 && e) atomicOr(&s_e, e);
         __syncthreads();
-        if (threadIdx.x == 0) p.flags[0] = s_e;
-        else if (threadIdx.x < 32) p.flags[threadIdx.x] = 0u;   // words 4..19: cycle counters of a GF_RENDER_TIMING build
+        if (threadIdx.x == 0) ws.flags[0] = s_e;
+        else if (threadIdx.x < 32) ws.flags[threadIdx.x] = 0u;   // words 4..19: cycle counters of a GF_RENDER_TIMING build
     }
 }
 
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
-int plan_forward_workspace(const gf_splat_desc &d, void *base, SplatWorkspace *ws) {
+SplatWorkspace plan_forward_workspace(const gf_splat_desc &d, WorkspaceCarver &carve) {
+    SplatWorkspace ws;
     // supertile edge in columns: a power of two and a multiple of both render bin edges (8 and 4)
     int st = 16;
     const size_t budget = size_t(512) << 20;
@@ -242,63 +228,33 @@ int plan_forward_workspace(const gf_splat_desc &d, void *base, SplatWorkspace *w
         if (ns * size_t(d.G) * 4 <= budget || st >= 1024) break;
         st *= 2;
     }
-    ws->st = st;
-    ws->nsx = (d.H + st - 1) / st;
-    ws->nsy = (d.W + st - 1) / st;
-    ws->nsuper = ws->nsx * ws->nsy;
-    ws->nwords = (d.G + 31) / 32;
-    ws->pack_ctas = (d.G + kPackThreads - 1) / kPackThreads;
-    const size_t B = static_cast<size_t>(batch_of(d));
-    ws->batch = static_cast<int>(B);
-    size_t off = 0;
-    char *b = static_cast<char *>(base);
-    auto take = [&](size_t bytes) {
-        char *p = b ? b + off : nullptr;
-        off = align_up(off + bytes, 256);
-        return p;
-    };
-    ws->flags = reinterpret_cast<uint32_t *>(take(256));
-    ws->pack_flags = reinterpret_cast<uint32_t *>(take(B * size_t(ws->pack_ctas) * 4));
-    ws->records = reinterpret_cast<float *>(take(B * size_t(d.G) * rec_floats(d.C) * 4));
-    ws->boxes = reinterpret_cast<PackedBox *>(take(B * size_t(d.G) * sizeof(PackedBox)));
-    ws->masks = reinterpret_cast<uint32_t *>(take(B * size_t(ws->nsuper) * ws->nwords * 4));
-    ws->lists = reinterpret_cast<int32_t *>(take(B * size_t(ws->nsuper) * d.G * 4));
-    ws->counts = reinterpret_cast<int32_t *>(take(B * size_t(ws->nsuper) * 4));
-    ws->bytes = off;
-    return GF_OK;
+    ws.rec = rec_floats(d.C);
+    ws.st = st;
+    ws.nsx = (d.H + st - 1) / st;
+    ws.nsy = (d.W + st - 1) / st;
+    ws.nsuper = ws.nsx * ws.nsy;
+    ws.nwords = (d.G + 31) / 32;
+    ws.pack_ctas = (d.G + kPackThreads - 1) / kPackThreads;
+    ws.batch = batch_of(d);
+    const size_t B = static_cast<size_t>(ws.batch);
+    ws.flags = carve.take<uint32_t>(256);
+    ws.pack_flags = carve.take<uint32_t>(B * ws.pack_ctas * 4);
+    ws.records = carve.take<float>(B * d.G * ws.rec * 4);
+    ws.boxes = carve.take<PackedBox>(B * d.G * sizeof(PackedBox));
+    ws.masks = carve.take<uint32_t>(B * ws.nsuper * ws.nwords * 4);
+    ws.lists = carve.take<int32_t>(B * ws.nsuper * d.G * 4);
+    ws.counts = carve.take<int32_t>(B * ws.nsuper * 4);
+    return ws;
 }
 
 int launch_prep(const gf_splat_desc &d, const gf_splat_inputs &in, const SplatWorkspace &ws,
                 uint32_t initial_flags, cudaStream_t stream, bool raw_records) {
-    PackParams pp;
-    pp.raw = raw_records ? 1 : 0;
-    pp.d = d;
-    pp.in = in;
-    pp.records = ws.records;
-    pp.boxes = ws.boxes;
-    pp.masks = ws.masks;
-    pp.pack_flags = ws.pack_flags;
-    pp.rec = rec_floats(d.C);
-    pp.st = ws.st;
-    pp.nsx = ws.nsx;
-    pp.nsy = ws.nsy;
-    pp.nwords = ws.nwords;
     if (ws.pack_ctas > 0) {
-        pack_mask_kernel<<<dim3(ws.pack_ctas, ws.batch), kPackThreads, 0, stream>>>(pp);
+        pack_mask_kernel<<<dim3(ws.pack_ctas, ws.batch), kPackThreads, 0, stream>>>(PackParams{d, in, ws, raw_records ? 1 : 0});
         GF_CUDA_TRY(cudaGetLastError());
     }
-    ListParams lp;
-    lp.masks = ws.masks;
-    lp.pack_flags = ws.pack_flags;
-    lp.lists = ws.lists;
-    lp.counts = ws.counts;
-    lp.flags = ws.flags;
-    lp.nwords = ws.nwords;
-    lp.G = d.G;
-    lp.pack_ctas = ws.pack_ctas * ws.batch;
-    lp.initial_flags = initial_flags;
     GF_REQUIRE(ws.batch <= 65535, GF_ERR_UNSUPPORTED, "splat: batch above 65535");
-    GF_CUDA_TRY(launch_chained(list_kernel, dim3(ws.nsuper, ws.batch), dim3(kListThreads), 0, stream, lp));
+    GF_CUDA_TRY(launch_chained(list_kernel, dim3(ws.nsuper, ws.batch), dim3(kListThreads), 0, stream, ListParams{ws, d.G, initial_flags}));
     return GF_OK;
 }
 

@@ -11,16 +11,10 @@ struct RenderParams {
     const float *pts;
     const int32_t *points_int;
     gf_splat_outputs out;
-    const float *records;
-    const PackedBox *boxes;
-    const int32_t *lists;
-    const int32_t *counts;
-    uint32_t *flags;
-    int st, nsy;     // supertile edge, supertiles along y
+    SplatWorkspace ws;
     int nby;         // bins along y
     int nzc;         // z chunks
     int nbx;         // bins along x (blockIdx.z = sample * nbx + bin x)
-    int nsuper;      // supertiles per sample
     int ce_rows;     // rows of out.ce_partials per sample (= render CTAs per sample)
     int vec_ok;      // D % 4 == 0 and every tensor the tile kernel touches with 16-byte vectors is 16-byte aligned
 };
@@ -35,14 +29,13 @@ __device__ __forceinline__ RenderParams with_sample_outputs(const RenderParams &
 }
 __device__ __forceinline__ RenderParams sample_params(const RenderParams &p, int b) {
     RenderParams q = p;
-    const long long G = p.d.G;
-    const long long np = p.d.pts_shared ? 0 : static_cast<long long>(b) * p.d.N * 3;
-    q.pts = p.pts + np;
-    q.points_int = adv(p.points_int, np);
-    q.records = p.records + static_cast<size_t>(b) * G * rec_floats(p.d.C);
-    q.boxes = p.boxes + static_cast<size_t>(b) * G;
-    q.lists = p.lists + static_cast<size_t>(b) * p.nsuper * G;
-    q.counts = p.counts + static_cast<size_t>(b) * p.nsuper;
+    gf_splat_inputs in = {};
+    in.pts = p.pts;
+    in.points_int = p.points_int;
+    in = sample_inputs(p.d, in, b);
+    q.pts = in.pts;
+    q.points_int = in.points_int;
+    q.ws = sample_ws(p.ws, p.d.G, b);
     return q;
 }
 
@@ -78,20 +71,20 @@ __device__ __forceinline__ void render_one_point(const RenderParams &p, long lon
     float zsum = 0.f, dens = 0.f, keep = 1.f;
     const bool ok = ix >= 0 && ix < H && iy >= 0 && iy < W && iz >= 0 && iz < D;
     if (!ok) {
-        atomicOr(p.flags, GF_FLAG_POINT_OUT_OF_GRID);
+        atomicOr(p.ws.flags, GF_FLAG_POINT_OUT_OF_GRID);
     } else {
-        const int s = (ix / p.st) * p.nsy + (iy / p.st);
-        const int ncand = p.counts[s];
-        const int32_t *cand = p.lists + static_cast<size_t>(s) * p.d.G;
+        const int s = supertile_of(p.ws, ix, iy);
+        const int ncand = p.ws.counts[s];
+        const int32_t *cand = p.ws.lists + static_cast<size_t>(s) * p.d.G;
         for (int i = 0; i < ncand; ++i) {
             const int g = __ldg(cand + i);
-            const uint4 b = __ldg(reinterpret_cast<const uint4 *>(p.boxes) + g);
+            const uint4 b = __ldg(reinterpret_cast<const uint4 *>(p.ws.boxes) + g);
             const bool in = static_cast<uint32_t>(ix) >= (b.x & 0xffffu) && static_cast<uint32_t>(ix) <= (b.x >> 16) &&
                             static_cast<uint32_t>(iy) >= (b.y & 0xffffu) && static_cast<uint32_t>(iy) <= (b.y >> 16) &&
                             static_cast<uint32_t>(iz) >= (b.z & 0xffffu) && static_cast<uint32_t>(iz) <= (b.z >> 16) &&
                             b.w == 0u;
             if (!in) continue;
-            const float4 *r4 = reinterpret_cast<const float4 *>(p.records + static_cast<size_t>(g) * REC);
+            const float4 *r4 = reinterpret_cast<const float4 *>(p.ws.records + static_cast<size_t>(g) * REC);
             const float4 g0 = __ldg(r4), g1 = __ldg(r4 + 1), g2 = __ldg(r4 + 2);
             const float dx = g0.x - x, dy = g0.y - y, dz = g0.z - z;
             float t1 = g1.x * dx;

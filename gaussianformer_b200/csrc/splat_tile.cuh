@@ -87,9 +87,8 @@ __device__ __forceinline__ void walk_tile(const RenderParams &p, RenderSmem<C> &
     // (the __syncthreads of Phase A below publishes the barrier initialisation)
 
     // ---- candidates: the ascending list of this bin's supertile ------------------------------------
-    const int st_shift = 31 - __clz(p.st);
-    const int s = (binX0 >> st_shift) * p.nsy + (binY0 >> st_shift);
-    const int ncand = p.counts[s];
+    const int s = supertile_of(p.ws, binX0, binY0);
+    const int ncand = p.ws.counts[s];
 
     int cpos = 0;
     while (cpos < ncand) {
@@ -98,8 +97,7 @@ __device__ __forceinline__ void walk_tile(const RenderParams &p, RenderSmem<C> &
         const long long tA0 = clock64();
 #endif
         // ======================= Phase A: ordered survivors of the box test ==========================
-        const int nlist = resolve_bin_list<NT, 4, kQuadSeg>(p.d, p.lists, s, ncand, cpos, p.boxes, binX0, binY0, binZ0, sm.list,
-                                                            sm.warp_count);
+        const int nlist = resolve_bin_list<NT, 4, kQuadSeg>(p.d, p.ws, s, ncand, cpos, binX0, binY0, binZ0, sm.list, sm.warp_count);
         // pad the last batch with empty entries (all-zero masks, so nobody visits them)
         if (tid < kBatch && nlist + tid < ((nlist + kBatch - 1) / kBatch) * kBatch) sm.list[nlist + tid] = make_uint2(0u, 0u);
         __syncthreads();
@@ -113,7 +111,7 @@ __device__ __forceinline__ void walk_tile(const RenderParams &p, RenderSmem<C> &
                 const int piece = tid + NT * q, row = piece >> 3, col = (piece & 7) * 4;
                 if (piece < kBatch * 8 && k * kBatch + row < nlist) {
                     const uint32_t g = sm.list[k * kBatch + row].y;
-                    cp_async16(&sm.stage[slot][row * ROW + col], p.records + static_cast<size_t>(g) * REC + col);
+                    cp_async16(&sm.stage[slot][row * ROW + col], p.ws.records + static_cast<size_t>(g) * REC + col);
                 }
             }
             cp_async_arrive_on(&sm.bar_full[slot]);
