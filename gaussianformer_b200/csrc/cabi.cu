@@ -285,7 +285,7 @@ int gf_daf_forward_ex(const gf_daf_desc *desc, int32_t feat_dtype, const void *f
     if (rc != GF_OK) return rc;
     DafParams p{};
     p.d = *desc; p.feat = feat; p.shape = shape; p.start = start; p.loc = loc; p.weights = weights; p.out = output;
-    return launch_daf(p, feat_dtype, false, num_sms, static_cast<cudaStream_t>(stream_));
+    return launch_daf(p, feat_dtype, DafPass::kForward, num_sms, static_cast<cudaStream_t>(stream_));
 }
 
 int gf_daf_backward(const gf_daf_desc *desc, const float *feat, const int32_t *shape, const int32_t *start,
@@ -352,7 +352,7 @@ int gf_daf_backward_ex2(const gf_daf_desc *desc, int32_t feat_dtype, uint32_t fl
     p.d = *desc; p.feat = feat; p.shape = shape; p.start = start; p.loc = loc; p.weights = weights;
     p.grad_out = grad_output; p.grad_feat = grad_feat; p.grad_loc = grad_loc; p.grad_weights = grad_weights;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    rc = launch_daf(p, feat_dtype, true, num_sms, stream, !det);
+    rc = launch_daf(p, feat_dtype, det ? DafPass::kBackwardNoFeatGrad : DafPass::kBackward, num_sms, stream);
     if (rc != GF_OK || !det) return rc;
     return launch_daf_det_feat_grad(&p, nullptr, workspace, num_sms, stream);
 }
@@ -400,7 +400,7 @@ int gf_daf_fused_forward_ex(const gf_daf_fused_desc *fd, int32_t feat_dtype, con
     DafFusedParams p{};
     p.d = fd->d; p.K = fd->pts_per_anchor; p.feat = feat; p.shape = shape; p.start = start; p.loc = loc; p.logits = logits;
     p.pmask = point_mask; p.wmask = weight_mask; p.out = output; p.stats = stats;
-    return launch_daf_fused(p, feat_dtype, false, num_sms, static_cast<cudaStream_t>(stream_));
+    return launch_daf_fused(p, feat_dtype, DafPass::kForward, num_sms, static_cast<cudaStream_t>(stream_));
 }
 
 int gf_daf_fused_backward(const gf_daf_fused_desc *fd, const float *feat, const int32_t *shape, const int32_t *start,
@@ -455,7 +455,7 @@ int gf_daf_fused_backward_ex2(const gf_daf_fused_desc *fd, int32_t feat_dtype, u
     p.pmask = point_mask; p.wmask = weight_mask; p.stats = const_cast<float *>(stats); p.out_saved = output;
     p.grad_out = grad_output; p.grad_feat = grad_feat; p.grad_loc = grad_loc; p.grad_logits = grad_logits;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    rc = launch_daf_fused(p, feat_dtype, true, num_sms, stream, !det);
+    rc = launch_daf_fused(p, feat_dtype, det ? DafPass::kBackwardNoFeatGrad : DafPass::kBackward, num_sms, stream);
     if (rc != GF_OK || !det) return rc;
     return launch_daf_det_feat_grad(nullptr, &p, workspace, num_sms, stream);
 }

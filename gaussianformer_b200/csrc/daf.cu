@@ -15,33 +15,6 @@
 
 namespace gf {
 
-struct Bilinear {
-    float w[4];          // corner weights (tl, tr, bl, br)
-    long long row[4];    // feature row of each corner inside the level
-    bool ok[4];
-    float lh, lw, hh, hw;
-};
-
-__device__ __forceinline__ Bilinear bilinear_setup(float lx, float ly, int h, int w) {
-    Bilinear b;
-    const float y_im = ly * static_cast<float>(h) - 0.5f;
-    const float x_im = lx * static_cast<float>(w) - 0.5f;
-    const float yf = floorf(y_im), xf = floorf(x_im);
-    const int y0 = static_cast<int>(yf), x0 = static_cast<int>(xf);
-    b.lh = y_im - yf; b.lw = x_im - xf;
-    b.hh = 1.f - b.lh; b.hw = 1.f - b.lw;
-    b.ok[0] = y0 >= 0 && x0 >= 0;
-    b.ok[1] = y0 >= 0 && x0 + 1 <= w - 1;
-    b.ok[2] = y0 + 1 <= h - 1 && x0 >= 0;
-    b.ok[3] = y0 + 1 <= h - 1 && x0 + 1 <= w - 1;
-    b.row[0] = static_cast<long long>(y0) * w + x0;
-    b.row[1] = b.row[0] + 1;
-    b.row[2] = b.row[0] + w;
-    b.row[3] = b.row[2] + 1;
-    b.w[0] = b.hh * b.hw; b.w[1] = b.hh * b.lw; b.w[2] = b.lh * b.hw; b.w[3] = b.lh * b.lw;
-    return b;
-}
-
 // Any C and Gr: a lane owns one channel per slice of 32 (shapes daf_fast_kernel does not take).
 template <bool BACKWARD, class T>
 __global__ void __launch_bounds__(kDafThreads) daf_kernel(const DafParams p) {
@@ -56,46 +29,40 @@ __global__ void __launch_bounds__(kDafThreads) daf_kernel(const DafParams p) {
 
     for (long long bp = static_cast<long long>(blockIdx.x) * (kDafThreads / 32) + (threadIdx.x >> 5); bp < npts; bp += warps) {
         const int b = static_cast<int>(bp / p.d.num_pts);
-        const float *locp = p.loc + bp * M * 2;  // (x,y) per camera; broadcast loads
         for (int c0 = lane; c0 < C; c0 += 32) {
             const int grp = c0 / gdim;
             float acc = 0.f;
             float gout = 0.f;
             if (BACKWARD) gout = __ldg(p.grad_out + bp * C + c0);
             for (int m = 0; m < M; ++m) {
-                const float lx = __ldg(locp + 2 * m), ly = __ldg(locp + 2 * m + 1);
-                if (!(lx > 0.f && lx < 1.f && ly > 0.f && ly < 1.f)) continue;  // warp-uniform
+                float lx, ly;
+                if (!cam_gate(p.loc, bp, M, m, lx, ly)) continue;  // warp-uniform
                 const T *fcam = feat + (static_cast<long long>(b) * M + m) * F * C + c0;
                 const long long wbase = (bp * M + m) * static_cast<long long>(L) * Gr + grp;
                 float gx = 0.f, gy = 0.f;
 #pragma unroll 4
                 for (int l = 0; l < L; ++l) {
-                    const Bilinear bl = bilinear_setup(lx, ly, lh[l], lw[l]);
+                    const BilinearCell cell = bilinear_cell(lx, ly, lh[l], lw[l]);
+                    const long long row0 = static_cast<long long>(cell.y0) * lw[l] + cell.x0;   // unclamped corner rows
+                    const long long row[4] = {row0, row0 + 1, row0 + lw[l], row0 + lw[l] + 1};
                     const T *flev = fcam + static_cast<long long>(ls[l]) * C;
                     float v[4];
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) v[k] = bl.ok[k] ? load1(flev + bl.row[k] * C) : 0.f;
+                    for (int k = 0; k < 4; ++k) v[k] = cell.inside(k, lh[l], lw[l]) ? load1(flev + row[k] * C) : 0.f;
                     const float wt = __ldg(p.weights + wbase + static_cast<long long>(l) * Gr);
+                    // d(out)/d(x_im), d(out)/d(y_im)   (cuda.cu:85-121)
+                    float dvx, dvy;
+                    const float val = bilinear_value(cell, v, dvx, dvy);
                     if (!BACKWARD) {
-                        float val = 0.f;
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) val = fmaf(bl.w[k], v[k], val);
                         acc = fmaf(wt, val, acc);
                     } else {
                         // d(out)/d(feat corner) = bilinear weight * aggregation weight
                         float *gf = p.grad_feat + (fcam - feat) + static_cast<long long>(ls[l]) * C;
 #pragma unroll
                         for (int k = 0; k < 4; ++k)
-                            if (bl.ok[k]) atomicAdd(gf + bl.row[k] * C, (bl.w[k] * wt) * gout);
+                            if (cell.inside(k, lh[l], lw[l])) atomicAdd(gf + row[k] * C, (cell.weight(k) * wt) * gout);
                         // d(out)/d(weight) = sampled value
-                        float val = 0.f;
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) val = fmaf(bl.w[k], v[k], val);
                         const float gw = gout * val;
-                        // d(out)/d(x_im), d(out)/d(y_im)   (cuda.cu:85-121)
-                        float dvx = 0.f, dvy = 0.f;
-                        dvx = fmaf(-bl.hh, v[0], dvx); dvx = fmaf(bl.hh, v[1], dvx); dvx = fmaf(-bl.lh, v[2], dvx); dvx = fmaf(bl.lh, v[3], dvx);
-                        dvy = fmaf(-bl.hw, v[0], dvy); dvy = fmaf(-bl.lw, v[1], dvy); dvy = fmaf(bl.hw, v[2], dvy); dvy = fmaf(bl.lw, v[3], dvy);
                         gx = fmaf(static_cast<float>(lw[l]) * wt, gout * dvx, gx);
                         gy = fmaf(static_cast<float>(lh[l]) * wt, gout * dvy, gy);
                         atomicAdd(p.grad_weights + wbase + static_cast<long long>(l) * Gr, gw);
@@ -129,16 +96,17 @@ __global__ void __launch_bounds__(kDafThreads) daf_det_generic_kernel(const DafP
 
     for (long long bp = static_cast<long long>(blockIdx.x) * (kDafThreads / 32) + (threadIdx.x >> 5); bp < npts; bp += warps) {
         const int b = static_cast<int>(bp / p.d.num_pts);
-        const float *locp = p.loc + bp * M * 2;
         const float *gop = p.grad_out + bp * C;
         for (int m = 0; m < M; ++m) {
-            const float lx = __ldg(locp + 2 * m), ly = __ldg(locp + 2 * m + 1);
-            if (!(lx > 0.f && lx < 1.f && ly > 0.f && ly < 1.f)) continue;  // warp-uniform
+            float lx, ly;
+            if (!cam_gate(p.loc, bp, M, m, lx, ly)) continue;  // warp-uniform
             const T *fcam = feat + (static_cast<long long>(b) * M + m) * F * C;
             const long long wbase = (bp * M + m) * static_cast<long long>(L) * Gr;
             float gx = 0.f, gy = 0.f;
             for (int l = 0; l < L; ++l) {
-                const Bilinear bl = bilinear_setup(lx, ly, lh[l], lw[l]);
+                const BilinearCell cell = bilinear_cell(lx, ly, lh[l], lw[l]);
+                const long long row0 = static_cast<long long>(cell.y0) * lw[l] + cell.x0;
+                const long long row[4] = {row0, row0 + 1, row0 + lw[l], row0 + lw[l] + 1};
                 const T *flev = fcam + static_cast<long long>(ls[l]) * C;
                 for (int g = lane; g < Gr; g += 32) {
                     const float wt = __ldg(p.weights + wbase + static_cast<long long>(l) * Gr + g);
@@ -146,15 +114,11 @@ __global__ void __launch_bounds__(kDafThreads) daf_det_generic_kernel(const DafP
                     for (int c = g * gdim; c < (g + 1) * gdim; ++c) {
                         float v[4];
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) v[k] = bl.ok[k] ? load1(flev + bl.row[k] * C + c) : 0.f;
+                        for (int k = 0; k < 4; ++k) v[k] = cell.inside(k, lh[l], lw[l]) ? load1(flev + row[k] * C + c) : 0.f;
                         const float gout = __ldg(gop + c);
-                        float val = 0.f;
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) val = fmaf(bl.w[k], v[k], val);
+                        float dvx, dvy;
+                        const float val = bilinear_value(cell, v, dvx, dvy);
                         gw = fmaf(gout, val, gw);
-                        float dvx = 0.f, dvy = 0.f;
-                        dvx = fmaf(-bl.hh, v[0], dvx); dvx = fmaf(bl.hh, v[1], dvx); dvx = fmaf(-bl.lh, v[2], dvx); dvx = fmaf(bl.lh, v[3], dvx);
-                        dvy = fmaf(-bl.hw, v[0], dvy); dvy = fmaf(-bl.lw, v[1], dvy); dvy = fmaf(bl.hw, v[2], dvy); dvy = fmaf(bl.lw, v[3], dvy);
                         gx = fmaf(static_cast<float>(lw[l]) * wt, gout * dvx, gx);
                         gy = fmaf(static_cast<float>(lh[l]) * wt, gout * dvy, gy);
                     }
@@ -217,22 +181,22 @@ __global__ void __launch_bounds__(kDafThreads, BACKWARD ? 3 : 4) daf_fast_kernel
     }
 }
 
-int launch_daf(const DafParams &p, int dtype, bool backward, int num_sms, cudaStream_t stream, bool feat_grad) {
+int launch_daf(const DafParams &p, int dtype, DafPass pass, int num_sms, cudaStream_t stream) {
     const long long npts = static_cast<long long>(p.d.batch) * p.d.num_pts;
     if (npts == 0) return GF_OK;
     const int grid = daf_grid(npts, num_sms);
     const bool v4 = daf_vec4_ok(p.d);
     return dispatch_feat_dtype(dtype, "daf", [&](auto tag) {
         using T = typename decltype(tag)::type;
-        if (backward && !feat_grad) {
-            if (v4) daf_fast_kernel<true, T, false><<<grid, kDafThreads, 0, stream>>>(p);
-            else daf_det_generic_kernel<T><<<grid, kDafThreads, 0, stream>>>(p);
-        } else if (backward) {
+        if (pass == DafPass::kForward) {
+            if (v4) daf_fast_kernel<false, T><<<grid, kDafThreads, 0, stream>>>(p);
+            else daf_kernel<false, T><<<grid, kDafThreads, 0, stream>>>(p);
+        } else if (pass == DafPass::kBackward) {
             if (v4) daf_fast_kernel<true, T><<<grid, kDafThreads, 0, stream>>>(p);
             else daf_kernel<true, T><<<grid, kDafThreads, 0, stream>>>(p);
         } else {
-            if (v4) daf_fast_kernel<false, T><<<grid, kDafThreads, 0, stream>>>(p);
-            else daf_kernel<false, T><<<grid, kDafThreads, 0, stream>>>(p);
+            if (v4) daf_fast_kernel<true, T, false><<<grid, kDafThreads, 0, stream>>>(p);
+            else daf_det_generic_kernel<T><<<grid, kDafThreads, 0, stream>>>(p);
         }
         GF_CUDA_TRY(cudaGetLastError());
         return GF_OK;

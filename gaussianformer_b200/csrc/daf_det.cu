@@ -182,13 +182,9 @@ __device__ __forceinline__ void load_det_levels(const DetParams &p, int *lh, int
     __syncthreads();
 }
 
-// the gate of the default kernels: camera m sees point bp (and, fused, the point mask lets it through)
+// camera m sees point bp (cam_gate) and, fused, the point mask lets it through
 __device__ __forceinline__ bool pair_visible(const DetParams &p, long long bp, int m, float &lx, float &ly) {
-    const long long at = (bp * p.d.num_cams + m) * 2;
-    lx = __ldg(p.loc + at);
-    ly = __ldg(p.loc + at + 1);
-    const bool gate = lx > 0.f && lx < 1.f && ly > 0.f && ly < 1.f;
-    return gate && (!p.pmask || p.pmask[bp * p.d.num_cams + m] != 0);
+    return cam_gate(p.loc, bp, p.d.num_cams, m, lx, ly) && (!p.pmask || p.pmask[bp * p.d.num_cams + m] != 0);
 }
 
 __global__ void __launch_bounds__(kDafThreads) det_count_kernel(const DetParams p) {
@@ -226,10 +222,8 @@ __global__ void __launch_bounds__(kDafThreads) det_emit_kernel(const DetParams p
             const uint32_t ballot = __ballot_sync(0xffffffffu, vis);
             if (vis) {
                 const int h = lh[l], w = lw[l];
-                // the corner cell exactly as pair_setup derives it
-                const int y0 = static_cast<int>(floorf(ly * static_cast<float>(h) - 0.5f));
-                const int x0 = static_cast<int>(floorf(lx * static_cast<float>(w) - 0.5f));
-                const long long key = (b * M + m) * p.cells_per_bm + le[l] + (y0 + 1) * (w + 1) + (x0 + 1);
+                const BilinearCell cell = bilinear_cell(lx, ly, h, w);   // the cell whose corners pair_setup reads
+                const long long key = (b * M + m) * p.cells_per_bm + le[l] + (cell.y0 + 1) * (w + 1) + (cell.x0 + 1);
                 const int at = pos + __popc(ballot & lanemask_lt());
                 p.keys[0][at] = static_cast<uint32_t>(key);
                 p.vals[0][at] = static_cast<int>(bp * npair + pr);
@@ -315,15 +309,14 @@ __global__ void __launch_bounds__(256) cell_bounds_kernel(const DetParams p, con
 }
 
 // ---------------------------------------------------------------------------------------------------------- gather
-// The aggregation weight of pair (bp, pr) for group grp, with the expression of the default kernels' weight callable
+// The aggregation weight of pair (bp, pr) for group grp: the plain op's weight, or the fused op's softmax_weight
 template <bool FUSED>
 __device__ __forceinline__ float pair_weight(const DetParams &p, long long bp, int pr, int grp, int npair) {
     const int Gr = p.d.num_groups;
     const long long widx = (bp * npair + pr) * Gr + grp;
     if (!FUSED) return __ldg(p.weights + widx);
     const float2 st = __ldg(reinterpret_cast<const float2 *>(p.stats + ((bp / p.K) * Gr + grp) * 2));
-    const float wt = ex2_approx(fmaf(__ldg(p.weights + widx), kLog2e, -st.x)) * st.y;
-    return (p.wmask && !p.wmask[widx]) ? 0.f : wt;
+    return softmax_weight(__ldg(p.weights + widx), st.x, st.y, p.wmask, widx);
 }
 
 // Adds the entries [i_beg, i_end) of one cell, whose corner k is the warp's row, to this lane's channel slice c0 (4
@@ -334,17 +327,13 @@ __device__ __forceinline__ void gather_cell(const DetParams &p, const int *vals,
                                             int h, int w, int c0, int grp, bool active, float4 &acc) {
     const int lane = threadIdx.x & 31, C = p.d.num_embeds, M = p.d.num_cams, L = p.d.num_scale, npair = M * L;
     for (int i0 = i_beg; i0 < i_end; i0 += 32) {
-        // lane e sets up entry i0 + e: its point and the bilinear weight of corner k, as pair_setup computes them
+        // lane e sets up entry i0 + e: its point and the bilinear weight of corner k of its cell (as in pair_setup)
         long long bp = 0;
         float cw = 0.f;
         if (i0 + lane < i_end) {
             bp = __ldg(vals + i0 + lane) / npair;
             const float *lp = p.loc + (bp * M + pr / L) * 2;
-            const float y_im = __ldg(lp + 1) * static_cast<float>(h) - 0.5f;
-            const float x_im = __ldg(lp) * static_cast<float>(w) - 0.5f;
-            const float lhh = y_im - floorf(y_im), lww = x_im - floorf(x_im);
-            const float hh = 1.f - lhh, hw = 1.f - lww;
-            cw = k == 0 ? hh * hw : k == 1 ? hh * lww : k == 2 ? lhh * hw : lhh * lww;
+            cw = bilinear_cell(__ldg(lp), __ldg(lp + 1), h, w).weight(k);
         }
         const int nb = min(32, i_end - i0);
         for (int e = 0; e < nb; ++e) {

@@ -64,7 +64,7 @@ __global__ void __launch_bounds__(kDafThreads, BACKWARD ? 3 : 4) daf_fused_kerne
             float sum = 0.f;
             for (int e = lane, it = 0; e < nE; e += 32, ++it) {
                 const bool on = (!pm || pm[pm_fast ? it * pm_step + pm_sub : e / LG]) && (!wm || wm[e]);
-                if (on) sum += ex2_approx(fmaf(__ldg(wl + e), kLog2e, -mlog));
+                if (on) sum += softmax_term(__ldg(wl + e), mlog);
             }
             for (int o = Gr; o < 32; o <<= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
             // a group with every entry masked ("all_miss", deformable_module.py:215-218,228) gets weight 0 everywhere
@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(kDafThreads, BACKWARD ? 3 : 4) daf_fused_kerne
             const float mlog = s_mlog[warp][eg], inv = s_inv[warp][eg], S = s_dot[warp][eg];
             for (int e = lane, it = 0; e < nE; e += 32, ++it) {
                 const bool on = (!pm || pm[pm_fast ? it * pm_step + pm_sub : e / LG]) && (!wm || wm[e]);
-                const float w = on ? ex2_approx(fmaf(__ldg(wl + e), kLog2e, -mlog)) * inv : 0.f;
+                const float w = on ? softmax_weight(__ldg(wl + e), mlog, inv, nullptr, e) : 0.f;   // on holds both masks
                 p.grad_logits[ba * nE + e] = -w * S;
             }
             __syncwarp();
@@ -120,11 +120,7 @@ __global__ void __launch_bounds__(kDafThreads, BACKWARD ? 3 : 4) daf_fused_kerne
                 const uint8_t *wmk = wm ? wm + k * npair * Gr : nullptr;
                 visit_pairs<BACKWARD, FEAT_GRAD>(
                     mine, visible, featb, gfeatb, c0, lane, lanes_per_group, gout, p.grad_loc, bp, M, acc,
-                    [=](int pr) {
-                        const int widx = pr * Gr + grp;
-                        const float wt = ex2_approx(fmaf(__ldg(wpt + widx), kLog2e, -mlog)) * inv;
-                        return (wmk && !wmk[widx]) ? 0.f : wt;       // select, never multiply: a masked logit may be anything
-                    },
+                    [=](int pr) { const int widx = pr * Gr + grp; return softmax_weight(__ldg(wpt + widx), mlog, inv, wmk, widx); },
                     // dL/dw_e = sampled value . g, then through the softmax
                     [glg = p.grad_logits, ba, nE, k, npair, Gr, grp, S](int pr, float wt, float gw) {
                         glg[ba * nE + static_cast<long long>(k) * npair * Gr + pr * Gr + grp] = wt * (gw - S);
@@ -145,15 +141,15 @@ bool daf_fused_supported(const gf_daf_desc &d, int K) {
     return static_cast<long long>(K) * d.num_cams * d.num_scale * Gr < (1ll << 31);
 }
 
-int launch_daf_fused(const DafFusedParams &p, int dtype, bool backward, int num_sms, cudaStream_t stream, bool feat_grad) {
+int launch_daf_fused(const DafFusedParams &p, int dtype, DafPass pass, int num_sms, cudaStream_t stream) {
     const long long nanchor = static_cast<long long>(p.d.batch) * (p.d.num_pts / p.K);
     if (nanchor == 0) return GF_OK;
     const int grid = daf_grid(nanchor, num_sms);
     return dispatch_feat_dtype(dtype, "daf fused", [&](auto tag) {
         using T = typename decltype(tag)::type;
-        if (backward && !feat_grad) daf_fused_kernel<true, T, false><<<grid, kDafThreads, 0, stream>>>(p);
-        else if (backward) daf_fused_kernel<true, T><<<grid, kDafThreads, 0, stream>>>(p);
-        else daf_fused_kernel<false, T><<<grid, kDafThreads, 0, stream>>>(p);
+        if (pass == DafPass::kForward) daf_fused_kernel<false, T><<<grid, kDafThreads, 0, stream>>>(p);
+        else if (pass == DafPass::kBackward) daf_fused_kernel<true, T><<<grid, kDafThreads, 0, stream>>>(p);
+        else daf_fused_kernel<true, T, false><<<grid, kDafThreads, 0, stream>>>(p);
         GF_CUDA_TRY(cudaGetLastError());
         return GF_OK;
     });

@@ -1,5 +1,6 @@
-// Pieces shared by the deformable-aggregation kernels (daf.cu, daf_fused.cu): their launch parameters, the level
-// table, and the one-warp-per-point visit of the fast kernels (daf_fast_kernel, daf_fused_kernel):
+// Pieces shared by the deformable-aggregation kernels (daf.cu, daf_fused.cu, daf_det.cu): their launch parameters, the
+// level table, the sampling arithmetic, and the one-warp-per-point visit of the fast kernels (daf_fast_kernel,
+// daf_fused_kernel):
 //   lane p < M*L      : pair p = (camera p / L, level p % L): gate, 4 corner rows (clamped to a valid row), 4 corner
 //                       weights (zero for corners outside the map) -> per-warp smem          (setup_pairs)
 //   ballot of the gate: only visible pairs are visited, in ascending (camera, level) order   (visit_pairs)
@@ -92,14 +93,16 @@ struct DafFusedParams {
     float *grad_feat, *grad_loc, *grad_logits;
 };
 
-// daf.cu (dtype: GF_DTYPE_* of the feature table / maps, checked by the caller).  feat_grad = false (backward only):
-// the weight and location gradients alone, each summed in an order fixed by the inputs (no floating-point atomics)
-int launch_daf(const DafParams &p, int dtype, bool backward, int num_sms, cudaStream_t stream, bool feat_grad = true);
+// What one launch of the sampling kernels computes.  kBackwardNoFeatGrad: the weight and location gradients alone, each
+// summed in an order fixed by the inputs (no floating-point atomics); daf_det.cu gathers the feature gradient.
+enum class DafPass { kForward, kBackward, kBackwardNoFeatGrad };
+
+// daf.cu (dtype: GF_DTYPE_* of the feature table / maps, checked by the caller)
+int launch_daf(const DafParams &p, int dtype, DafPass pass, int num_sms, cudaStream_t stream);
 int launch_daf_format(const gf_daf_format_desc &d, int dtype, void *const *maps, void *table, bool inverse, cudaStream_t stream);
 // daf_fused.cu
 bool daf_fused_supported(const gf_daf_desc &d, int K);
-int launch_daf_fused(const DafFusedParams &p, int dtype, bool backward, int num_sms, cudaStream_t stream,
-                     bool feat_grad = true);
+int launch_daf_fused(const DafFusedParams &p, int dtype, DafPass pass, int num_sms, cudaStream_t stream);
 // daf_det.cu: the ordered feature gradient of the deterministic backward (GF_BWD_DETERMINISTIC).
 // daf_det_workspace_bytes: 0 with a message when the desc is outside the route's limits.  launch_daf_det_feat_grad
 // adds (+=) the feature gradient of the plain op (fp = nullptr) or of the fused one (p = nullptr) into grad_feat.
@@ -129,29 +132,76 @@ __device__ __forceinline__ void load_level_table(const gf_daf_desc &d, const int
     __syncthreads();
 }
 
+// ---- The sampling arithmetic of every DAF kernel: the camera gate, the bilinear cell with its corner weights and
+// the fused op's softmax weight.  The deterministic backward (daf_det.cu) re-derives the cells and coefficients of the
+// default kernels and is exact only while both evaluate the same expressions, so every kernel calls these functions
+// instead of restating them.  nvcc contracts multiply/add pairs: operand order is part of each definition.
+
+// Location (lx, ly) of point bp in camera m, and the gate: the camera sees the point strictly inside (0, 1)^2.
+__device__ __forceinline__ bool cam_gate(const float *loc, long long bp, int M, int m, float &lx, float &ly) {
+    lx = __ldg(loc + (bp * M + m) * 2); ly = __ldg(loc + (bp * M + m) * 2 + 1);
+    return lx > 0.f && lx < 1.f && ly > 0.f && ly < 1.f;
+}
+
+// The bilinear cell of a location on an h x w map (pixel centres at +0.5): its unclamped top-left corner (y0, x0),
+// the fractional parts lh, lw and their complements hh, hw.  Corner k is (y0 + k/2, x0 + k%2).
+struct BilinearCell {
+    int y0, x0;
+    float lh, lw, hh, hw;
+    __device__ __forceinline__ float weight(int k) const { return k == 0 ? hh * hw : k == 1 ? hh * lw : k == 2 ? lh * hw : lh * lw; }
+    // row y0 + dy / column x0 + dx (dy, dx = 0 or 1) lies inside the h x w map, and so does corner k
+    __device__ __forceinline__ bool row_inside(int dy, int h) const { return dy ? y0 + 1 <= h - 1 : y0 >= 0; }
+    __device__ __forceinline__ bool col_inside(int dx, int w) const { return dx ? x0 + 1 <= w - 1 : x0 >= 0; }
+    __device__ __forceinline__ bool inside(int k, int h, int w) const { return row_inside(k >> 1, h) && col_inside(k & 1, w); }
+};
+
+__device__ __forceinline__ BilinearCell bilinear_cell(float lx, float ly, int h, int w) {
+    const float y_im = ly * static_cast<float>(h) - 0.5f, x_im = lx * static_cast<float>(w) - 0.5f;
+    const float yf = floorf(y_im), xf = floorf(x_im), lh = y_im - yf, lw = x_im - xf;
+    return {static_cast<int>(yf), static_cast<int>(xf), lh, lw, 1.f - lh, 1.f - lw};
+}
+
+// The scalar kernels' step (daf_kernel, daf_det_generic_kernel): the bilinear value of the corner values v (0 for
+// corners outside the map) and its derivatives along x_im and y_im.
+__device__ __forceinline__ float bilinear_value(const BilinearCell &c, const float v[4], float &dvx, float &dvy) {
+    float val = 0.f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) val = fmaf(c.weight(k), v[k], val);
+    dvx = fmaf(-c.hh, v[0], 0.f); dvx = fmaf(c.hh, v[1], dvx); dvx = fmaf(-c.lh, v[2], dvx); dvx = fmaf(c.lh, v[3], dvx);
+    dvy = fmaf(-c.hw, v[0], 0.f); dvy = fmaf(-c.lw, v[1], dvy); dvy = fmaf(c.hw, v[2], dvy); dvy = fmaf(c.lw, v[3], dvy);
+    return val;
+}
+
+// The fused op's softmax term exp2(logit * log2e - mlog) (mlog = the group's max * log2e), and the weight term / sum
+// (inv = 1 / sum) of entry i, 0 where the weight mask wm (NULL: none) is off: a select, never a multiply, since a
+// masked logit may be anything.
+__device__ __forceinline__ float softmax_term(float logit, float mlog) { return ex2_approx(fmaf(logit, kLog2e, -mlog)); }
+template <class I>
+__device__ __forceinline__ float softmax_weight(float logit, float mlog, float inv, const uint8_t *wm, I i) {
+    const float wt = softmax_term(logit, mlog) * inv;
+    return (wm && !wm[i]) ? 0.f : wt;
+}
+
 __device__ __forceinline__ bool pair_setup(const gf_daf_desc &d, const float *loc, const int *lh, const int *lw, const int *ls,
                                            long long bp, int m, int lv, PairSetup &o) {
     const int M = d.num_cams, F = d.num_feat, C = d.num_embeds;
-    const float lx = __ldg(loc + (bp * M + m) * 2), ly = __ldg(loc + (bp * M + m) * 2 + 1);
-    const bool gate = lx > 0.f && lx < 1.f && ly > 0.f && ly < 1.f;
+    float lx, ly;
+    const bool gate = cam_gate(loc, bp, M, m, lx, ly);
     const int h = lh[lv], w = lw[lv];
-    const float y_im = ly * static_cast<float>(h) - 0.5f, x_im = lx * static_cast<float>(w) - 0.5f;
-    const float yf = floorf(y_im), xf = floorf(x_im);
-    const int y0 = static_cast<int>(yf), x0 = static_cast<int>(xf);
-    o.lh = y_im - yf; o.lw = x_im - xf;
+    const BilinearCell cell = bilinear_cell(lx, ly, h, w);
+    o.lh = cell.lh; o.lw = cell.lw;
     o.fh = static_cast<float>(h); o.fw = static_cast<float>(w);
-    const float hh = 1.f - o.lh, hw = 1.f - o.lw;
-    const bool oky0 = y0 >= 0, oky1 = y0 + 1 <= h - 1, okx0 = x0 >= 0, okx1 = x0 + 1 <= w - 1;
-    const int cy0 = max(y0, 0), cy1 = min(y0 + 1, h - 1), cx0 = max(x0, 0), cx1 = min(x0 + 1, w - 1);
+    const bool oky0 = cell.row_inside(0, h), oky1 = cell.row_inside(1, h), okx0 = cell.col_inside(0, w), okx1 = cell.col_inside(1, w);
+    const int cy0 = max(cell.y0, 0), cy1 = min(cell.y0 + 1, h - 1), cx0 = max(cell.x0, 0), cx1 = min(cell.x0 + 1, w - 1);
     const int base = m * F + ls[lv];
     o.row[0] = (base + cy0 * w + cx0) * C;
     o.row[1] = (base + cy0 * w + cx1) * C;
     o.row[2] = (base + cy1 * w + cx0) * C;
     o.row[3] = (base + cy1 * w + cx1) * C;
-    o.w[0] = (oky0 && okx0) ? hh * hw : 0.f;
-    o.w[1] = (oky0 && okx1) ? hh * o.lw : 0.f;
-    o.w[2] = (oky1 && okx0) ? o.lh * hw : 0.f;
-    o.w[3] = (oky1 && okx1) ? o.lh * o.lw : 0.f;
+    o.w[0] = (oky0 && okx0) ? cell.weight(0) : 0.f;
+    o.w[1] = (oky0 && okx1) ? cell.weight(1) : 0.f;
+    o.w[2] = (oky1 && okx0) ? cell.weight(2) : 0.f;
+    o.w[3] = (oky1 && okx1) ? cell.weight(3) : 0.f;
     o.ok = (oky0 && okx0 ? 1 : 0) | (oky0 && okx1 ? 2 : 0) | (oky1 && okx0 ? 4 : 0) | (oky1 && okx1 ? 8 : 0);
     o.cam = m;
     o.pad0 = o.pad1 = 0;
