@@ -123,6 +123,10 @@ __global__ void __launch_bounds__(kRenderThreads, PROB ? 3 : 4) render_tile_kern
     // come from the two preparation kernels, which this grid may have been launched ahead of.
     pdl_wait();
     if (stray) atomicOr(pin.ws.flags, GF_FLAG_GENERIC_PATH);
+    {
+        const bool warp_stray = __any_sync(0xffffffffu, stray != 0);   // read by the epilogue; kept out of registers
+        if (lane == 0) sm.stray_warp[warp] = warp_stray;
+    }
 #ifdef GF_RENDER_TIMING
     if (tid == 0) sm.t_phase[0] = static_cast<unsigned long long>(clock64() - t_start);
 #endif
@@ -294,9 +298,44 @@ __global__ void __launch_bounds__(kRenderThreads, PROB ? 3 : 4) render_tile_kern
             p.out.ce_partials[2 * cta + 1] = b;
         }
     }
+    // [N, C] logits through the shared tile and bulk copies when that writes exactly what the direct stores would:
+    // 16-byte aligned rows, whole z chunks (each column of the bin is then one contiguous run of kBinZ * C floats) and
+    // no stray point in the CTA (render_one_point overwrites a stray row with ordinary stores after the direct ones).
+    // A thread's direct stores would touch 32 lines per warp instruction at a 4*C*4-byte stride; the copies write
+    // whole lines, and the CTA exits once the tile has been read instead of after issuing every store.
+    bool bulk = p.out.logits && vec_ok && D % kBinZ == 0;
+    if (bulk) {
+        __syncthreads();   // every warp is done with the walk buffers the tile overwrites
+        uint32_t any_stray = 0;
+#pragma unroll
+        for (int w = 0; w < kRenderThreads / 32; ++w) any_stray |= sm.stray_warp[w];
+        bulk = any_stray == 0;
+    }
+    if (bulk) {
+        if (live) {
+            float *dst = &sm.tile[lx * kBinY + ly][VOX * C * lq];
+            float flat[VOX * C];
+#pragma unroll
+            for (int v = 0; v < VOX; ++v)
+#pragma unroll
+                for (int c = 0; c < C; ++c) flat[v * C + c] = out[v][c];
+#pragma unroll
+            for (int i = 0; i < VOX * C / 4; ++i)
+                st_shared16(dst + 4 * i, make_float4(flat[4 * i], flat[4 * i + 1], flat[4 * i + 2], flat[4 * i + 3]));
+        }
+        fence_proxy_async_shared();
+        __syncthreads();
+        if (warp == 0) {   // lane l copies column l of the bin
+            const int cx = binX0 + lane / kBinY, cy = binY0 + lane % kBinY;
+            if (cx < H && cy < W)
+                bulk_copy_s2g(p.out.logits + ((static_cast<long long>(cx) * W + cy) * D + binZ0) * C, &sm.tile[lane][0],
+                              kBinZ * C * sizeof(float));
+            bulk_commit_wait_read();
+        }
+    }
     if (live) {
         if (vec_ok) {
-            if (p.out.logits) {
+            if (p.out.logits && !bulk) {
                 float *dst = p.out.logits + n0 * C;
                 float flat[VOX * C];
 #pragma unroll

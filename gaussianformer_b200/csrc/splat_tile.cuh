@@ -22,13 +22,24 @@ struct RenderSmem {
     static constexpr int REC = rec_floats(C);
     static constexpr int ROW = REC + 4;        // floats per staged row
     static constexpr int NT = kRenderThreads;
-    alignas(128) float stage[kRing][kBatch * ROW];
-    alignas(8) uint2 list[kQuadSeg + kBatch];  // x: box relative to the bin as bit masks, y: Gaussian index
-    uint32_t hitw[kQuadSeg / kBatch + 1][16];  // per batch: bit j of word i = entry j covers x position i (0..7), y position i-8 (8..11), z quad i-12 (12..15)
+    // Epilogue tile: the CTA's logits in [N, C] order, one row of kBinZ voxels per column (x-major), each row padded
+    // by 16 bytes so that the two z quads of neighbouring lanes fall into different bank groups.  A row is one
+    // contiguous run of the output when D % kBinZ == 0, copied out with one bulk copy.
+    static constexpr int TILE_ROW = kBinZ * C + 4;
+    struct Walk {
+        alignas(128) float stage[kRing][kBatch * ROW];
+        alignas(8) uint2 list[kQuadSeg + kBatch];  // x: box relative to the bin as bit masks, y: Gaussian index
+        uint32_t hitw[kQuadSeg / kBatch + 1][16];  // per batch: bit j of word i = entry j covers x position i (0..7), y position i-8 (8..11), z quad i-12 (12..15)
+    };
+    union {
+        Walk w;                                              // Phase A and B
+        alignas(128) float tile[kBinX * kBinY][TILE_ROW];    // epilogue: the walk's buffers are dead by then
+    };
     alignas(8) uint64_t bar_full[kRing];       // records of the slot have landed (one cp.async arrival per thread)
     alignas(8) uint64_t bar_empty[kRing];      // every warp is done with the slot (one arrival per warp)
     int warp_count[2][NT / 32];
     float ce[NT / 32][2];                      // per-warp cross-entropy partials of the epilogue
+    uint32_t stray_warp[NT / 32];              // per warp: some lane has a point outside canonical voxel order
 #ifdef GF_RENDER_TIMING
     unsigned long long t_phase[8];             // cycle sums: prologue, Phase A, Phase B, epilogue (thread 0); all warps: wait-full, wait-empty + issue, hit masks, walk
 #endif
@@ -43,6 +54,22 @@ __device__ __forceinline__ void cp_async_arrive_on(uint64_t *bar) {
 }
 __device__ __forceinline__ void mbar_arrive_one(uint64_t *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void st_shared16(void *smem_dst, float4 v) {
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(smem_u32(smem_dst)), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
+                 : "memory");
+}
+// this thread's shared-memory writes become visible to the bulk copies (async proxy) issued after the next barrier
+__device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// bulk copy of `bytes` (a multiple of 16, both addresses 16-byte aligned) from shared to global memory
+__device__ __forceinline__ void bulk_copy_s2g(void *gmem_dst, const void *smem_src, uint32_t bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gmem_dst), "r"(smem_u32(smem_src)), "r"(bytes)
+                 : "memory");
+}
+// commit this thread's bulk copies and wait until they have READ their shared-memory sources; the global writes drain
+// on their own and are visible to later kernels of the stream
+__device__ __forceinline__ void bulk_commit_wait_read() {
+    asm volatile("cp.async.bulk.commit_group;\n\tcp.async.bulk.wait_group.read 0;" ::: "memory");
 }
 
 // One staged record as a lane sees it: `addr` is the shared-space address of its row, chunk i sits 16*i bytes further.
@@ -97,9 +124,9 @@ __device__ __forceinline__ void walk_tile(const RenderParams &p, RenderSmem<C> &
         const long long tA0 = clock64();
 #endif
         // ======================= Phase A: ordered survivors of the box test ==========================
-        const int nlist = resolve_bin_list<NT, 4, kQuadSeg>(p.d, p.ws, s, ncand, cpos, binX0, binY0, binZ0, sm.list, sm.warp_count);
+        const int nlist = resolve_bin_list<NT, 4, kQuadSeg>(p.d, p.ws, s, ncand, cpos, binX0, binY0, binZ0, sm.w.list, sm.warp_count);
         // pad the last batch with empty entries (all-zero masks, so nobody visits them)
-        if (tid < kBatch && nlist + tid < ((nlist + kBatch - 1) / kBatch) * kBatch) sm.list[nlist + tid] = make_uint2(0u, 0u);
+        if (tid < kBatch && nlist + tid < ((nlist + kBatch - 1) / kBatch) * kBatch) sm.w.list[nlist + tid] = make_uint2(0u, 0u);
         __syncthreads();
         const int nchunks = (nlist + kBatch - 1) / kBatch;
         auto issue = [&](int k, uint32_t b_index) {  // batch k of this segment -> ring slot b_index % kRing
@@ -110,8 +137,8 @@ __device__ __forceinline__ void walk_tile(const RenderParams &p, RenderSmem<C> &
             for (int q = 0; q < (kBatch * 8 + NT - 1) / NT; ++q) {     // 32 records x 8 x 16 B = 256 copies
                 const int piece = tid + NT * q, row = piece >> 3, col = (piece & 7) * 4;
                 if (piece < kBatch * 8 && k * kBatch + row < nlist) {
-                    const uint32_t g = sm.list[k * kBatch + row].y;
-                    cp_async16(&sm.stage[slot][row * ROW + col], p.ws.records + static_cast<size_t>(g) * REC + col);
+                    const uint32_t g = sm.w.list[k * kBatch + row].y;
+                    cp_async16(&sm.w.stage[slot][row * ROW + col], p.ws.records + static_cast<size_t>(g) * REC + col);
                 }
             }
             cp_async_arrive_on(&sm.bar_full[slot]);
@@ -122,7 +149,7 @@ __device__ __forceinline__ void walk_tile(const RenderParams &p, RenderSmem<C> &
         // transpose them into 16 words (which entries cover x position i / y position i / z quad i); a lane's hit mask of a
         // batch is then the AND of three of those words (ten ballots per warp and batch before: 9 % of Phase B).
         for (int b = warp; b < (nlist + kBatch - 1) / kBatch; b += NWARP) {
-            const uint32_t ex = sm.list[b * kBatch + lane].x;
+            const uint32_t ex = sm.w.list[b * kBatch + lane].x;
             uint32_t mine = 0u;
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
@@ -130,7 +157,7 @@ __device__ __forceinline__ void walk_tile(const RenderParams &p, RenderSmem<C> &
                 const uint32_t w = __ballot_sync(0xffffffffu, covers);
                 if (lane == i) mine = w;
             }
-            if (lane < 16) sm.hitw[b][lane] = mine;
+            if (lane < 16) sm.w.hitw[b][lane] = mine;
         }
         __syncthreads();
 #ifdef GF_RENDER_TIMING
@@ -147,11 +174,11 @@ __device__ __forceinline__ void walk_tile(const RenderParams &p, RenderSmem<C> &
             const long long tk0 = clock64();
 #endif
             const int slot = gb % kRing;
-            const uint32_t stage_base = smem_u32(&sm.stage[slot][0]);
+            const uint32_t stage_base = smem_u32(&sm.w.stage[slot][0]);
             // bit j of `hits`: record j of this batch covers my column and my z quad (padded entries are all-zero)
             uint32_t hits;
             {
-                const uint32_t *hw = sm.hitw[k];
+                const uint32_t *hw = sm.w.hitw[k];
                 hits = hw[4 * (warp & 1) + (lane >> 3)] & hw[8 + ((lane >> 1) & 3)] & hw[12 + 2 * (warp >> 1) + (lane & 1)];
             }
 #ifdef GF_RENDER_TIMING
@@ -168,7 +195,7 @@ __device__ __forceinline__ void walk_tile(const RenderParams &p, RenderSmem<C> &
                 const int jraw = __ffs(static_cast<int>(hits)) - 1;          // my lowest remaining hit; -1 when I have none
                 hits &= hits - 1;                                             // 0 stays 0
                 rv.addr = stage_base + static_cast<uint32_t>(jraw * (ROW * 4));   // an inactive lane never dereferences it
-                const uint32_t e = sm.list[k * kBatch + (act ? jraw : 0)].x;
+                const uint32_t e = sm.w.list[k * kBatch + (act ? jraw : 0)].x;
                 zb = (e >> my_zshift) & VMASK;
             };
             if (fast) {
