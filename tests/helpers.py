@@ -62,14 +62,24 @@ def to_dev(inp, device="cuda", requires_grad=False):
     return t
 
 
+def outside_tolerance(actual, expected, tol):
+    """(mask of the entries with |actual - expected| > tol, |actual - expected|, index of the worst one or None).  A NaN
+    or an infinity is outside unless both sides hold the same value: ``err > tol`` alone is False for a NaN, so a kernel
+    that leaves rows unwritten or sums uninitialised memory would pass."""
+    with np.errstate(invalid="ignore"):   # inf - inf
+        err = np.abs(actual - expected)
+        bad = ~((err <= tol) | (actual == expected) | (np.isnan(actual) & np.isnan(expected)))
+    if not bad.any():
+        return bad, err, None
+    return bad, err, np.unravel_index(np.argmax(np.where(bad, np.nan_to_num(err - tol, nan=np.inf), -np.inf)), err.shape)
+
+
 def assert_close(actual, expected, rtol=RTOL, atol=ATOL, what=""):
     actual = np.asarray(actual, dtype=np.float64)
     expected = np.asarray(expected, dtype=np.float64)
-    err = np.abs(actual - expected)
     tol = atol + rtol * np.abs(expected)
-    bad = err > tol
+    bad, err, i = outside_tolerance(actual, expected, tol)
     if bad.any():
-        i = np.unravel_index(np.argmax(err - tol), err.shape)
         raise AssertionError(f"{what}: {int(bad.sum())}/{bad.size} outside tolerance; worst at {i}: "
                              f"got {actual[i]!r} want {expected[i]!r} (|err|={err[i]:.3e}, tol={tol[i]:.3e})")
 
@@ -94,12 +104,10 @@ def assert_grad_parity(mine, ref64, ref32, what="", k=K_FLOOR, extra_floor=0.0):
     1-20x CLOSER to the fp64 oracle than the reference op."""
     mine = np.asarray(mine, np.float64)
     ref64 = np.asarray(ref64, np.float64)
-    err = np.abs(mine - ref64)
     floor = max(float(np.abs(np.asarray(ref32, np.float64) - ref64).max()), float(extra_floor))
     tol = np.maximum(ATOL + RTOL * np.abs(ref64), k * floor)
-    bad = err > tol
+    bad, err, i = outside_tolerance(mine, ref64, tol)
     if bad.any():
-        i = np.unravel_index(np.argmax(err - tol), err.shape)
         raise AssertionError(f"{what}: {int(bad.sum())}/{bad.size} outside max(1e-5 + 1e-4|ref|, {k} x fp32 floor {floor:.3e}); "
                              f"worst at {i}: got {mine[i]!r} want {ref64[i]!r} (|err|={err[i]:.3e})")
 

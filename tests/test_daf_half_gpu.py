@@ -37,10 +37,8 @@ def assert_half_grad(mine, ref64, ref32, dtype, what):
     ref64 = np.asarray(ref64, np.float64)
     floor = float(np.abs(np.asarray(ref32, np.float64) - ref64).max())
     tol = np.maximum(h.ATOL + h.RTOL * np.abs(ref64), h.K_FLOOR * floor) + _ulp(ref64, dtype)
-    err = np.abs(mine - ref64)
-    bad = err > tol
+    bad, _, i = h.outside_tolerance(mine, ref64, tol)
     if bad.any():
-        i = np.unravel_index(np.argmax(err - tol), err.shape)
         raise AssertionError(f"{what}: {int(bad.sum())}/{bad.size} outside the fp32 gate + 1 ulp; worst at {i}: "
                              f"got {mine[i]!r} want {ref64[i]!r}")
 

@@ -173,12 +173,13 @@ def test_sample_alone_equals_sample_in_batch(variant, permuted):
 
 # ------------------------------------------------------------------------------------------------ hooks
 def _route_words(kw, inp, variant):
-    """one deterministic backward through splat_backward_raw with our own workspace; its route word per sample"""
+    """one deterministic backward through splat_backward_raw with our own workspace; its route word per sample
+    (``inp["pts"]`` [N, 3]: one point array shared by the batch)"""
     from gaussianformer_b200.splat import _desc_for, splat_backward_raw, splat_forward_raw
     m = h.make_module(kw, variant)
     t = h.to_dev(inp)
     B, G = t["means"].shape[:2]
-    desc = _desc_for(m._cfg(), B, G, t["pts"].shape[1], t["sem"].shape[-1], False)
+    desc = _desc_for(m._cfg(), B, G, t["pts"].shape[-2], t["sem"].shape[-1], t["pts"].dim() == 2)
     cov = t["cov"].reshape(B, G, 9).contiguous()
     (lg, bl, de, pr), _ = splat_forward_raw(desc, t["pts"], t["means"], t["opa"], t["sem"], cov, scales=t["scales"])
     gen = torch.Generator(device="cuda").manual_seed(3)
