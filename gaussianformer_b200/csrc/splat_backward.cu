@@ -324,22 +324,11 @@ __global__ void __launch_bounds__(128) srt_grad_kernel(const BwdParams pb) {
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-struct BwdWorkspace {
-    int32_t *v2p, *canon;
-    unsigned long long *big_ctr;
-    uint2 *big;
-    float4 *aux;
-    float *cov6;       // [B,G,6] gradient of Sigma^-1 when the caller passed scales + rotations instead of cov
-    SplatWorkspace fwd;   // records, boxes and supertile lists for the bin-centric kernel
-    float *sums;       // [B,G,32] raw sums of the bin-centric kernel
-    size_t sums_bytes;
-    size_t cv_block;   // bytes of one sample's (canon word, voxel -> point map) block
-    size_t cv_bytes;   // all of them: one memset
-    // deterministic mode only (carved behind everything above, so the layout without the flag is unchanged)
-    BinSlots slots;    // the bin kernel's per-(Gaussian, bin) slots
-    uint32_t *det_cnt; // [B,G] chunk counts of the queued boxes
-    float *det_part;   // [B,G+kDetBigCtas,32] segment sums of the big kernel
-    size_t bytes;
+// Byte counts of the backward workspace that only the host needs.
+struct BwdPlan {
+    size_t cv_bytes;     // the (canon word, voxel -> point map) blocks of all samples: one memset
+    size_t sums_bytes;   // BwdParams::sums: one memset
+    size_t bytes;        // the whole workspace
 };
 
 // Box voxels per chunk of the big-box kernel: 4 passes of a 256-thread CTA, grown when needed so that
@@ -363,54 +352,52 @@ static long long slot_budget(const gf_splat_desc &d) {
     return b < 0xffffffffll ? b : 0xffffffffll;   // slot numbers are 32-bit
 }
 
-void plan_backward_workspace(const gf_splat_desc &d, uint32_t flags, void *base, BwdWorkspace *ws) {
+// Carves the workspace at `base` (nullptr: only sizes it) into the workspace fields of ws.
+BwdPlan plan_backward_workspace(const gf_splat_desc &d, uint32_t flags, void *base, BwdParams &ws) {
     WorkspaceCarver carve{static_cast<char *>(base)};
     const size_t B = static_cast<size_t>(batch_of(d));
-    ws->big_ctr = carve.take<unsigned long long>(B * 8);
-    // per sample: the canon word (256 bytes) directly in front of its voxel -> point map; one memset covers all
-    ws->cv_block = 256 + WorkspaceCarver::align(size_t(d.H) * d.W * d.D * 4);
-    ws->cv_bytes = B * ws->cv_block;
-    ws->canon = carve.take<int32_t>(ws->cv_bytes);
-    ws->v2p = ws->canon ? ws->canon + 64 : nullptr;
-    ws->big = carve.take<uint2>(B * size_t(d.G) * sizeof(uint2));
-    ws->aux = carve.take<float4>(d.variant == GF_SPLAT_PROB ? B * size_t(d.N) * 16 : 0);
-    ws->cov6 = carve.take<float>(B * size_t(d.G) * 6 * 4);   // only used with scales + rotations input
-    ws->fwd = plan_forward_workspace(d, carve);
-    ws->sums_bytes = B * size_t(d.G) * 32 * 4;
-    ws->sums = carve.take<float>(ws->sums_bytes);
-    ws->slots = BinSlots{nullptr, nullptr, 0};
-    ws->det_cnt = nullptr;
-    ws->det_part = nullptr;
-    if (flags & GF_BWD_DETERMINISTIC) {
-        ws->slots.budget = slot_budget(d);
-        ws->slots.slot_off = carve.take<uint32_t>(B * size_t(d.G) * 4);
-        ws->slots.slots = carve.take<float>(B * size_t(ws->slots.budget) * 32 * 4);
-        ws->det_cnt = carve.take<uint32_t>(B * size_t(d.G) * 4);
-        ws->det_part = carve.take<float>(B * (size_t(d.G) + kDetBigCtas) * 32 * 4);
-    }
-    ws->bytes = carve.bytes;
+    BwdPlan plan;
+    ws.big_ctr = carve.take<unsigned long long>(B * 8);
+    ws.cv_block = 256 + WorkspaceCarver::align(size_t(d.H) * d.W * d.D * 4);
+    plan.cv_bytes = B * ws.cv_block;
+    ws.canon = carve.take<int32_t>(plan.cv_bytes);
+    ws.v2p = ws.canon ? ws.canon + 64 : nullptr;
+    ws.big = carve.take<uint2>(B * size_t(d.G) * sizeof(uint2));
+    ws.chunk = chunk_voxels(d);
+    ws.aux = carve.take<float4>(d.variant == GF_SPLAT_PROB ? B * size_t(d.N) * 16 : 0);
+    ws.cov6 = carve.take<float>(B * size_t(d.G) * 6 * 4);   // only used with scales + rotations input
+    ws.fwd = plan_forward_workspace(d, carve);
+    plan.sums_bytes = B * size_t(d.G) * 32 * 4;
+    ws.sums = carve.take<float>(plan.sums_bytes);
+    const bool det = (flags & GF_BWD_DETERMINISTIC) != 0;
+    ws.budget = det ? slot_budget(d) : 0;
+    ws.slot_off = det ? carve.take<uint32_t>(B * size_t(d.G) * 4) : nullptr;
+    ws.slots = det ? carve.take<float>(B * size_t(ws.budget) * 32 * 4) : nullptr;
+    ws.det_cnt = det ? carve.take<uint32_t>(B * size_t(d.G) * 4) : nullptr;
+    ws.det_part = det ? carve.take<float>(B * (size_t(d.G) + kDetBigCtas) * 32 * 4) : nullptr;
+    plan.bytes = carve.bytes;
+    return plan;
 }
 
 size_t backward_workspace_bytes(const gf_splat_desc &d, uint32_t flags) {
-    BwdWorkspace ws;
-    plan_backward_workspace(d, flags, nullptr, &ws);
-    return ws.bytes;
+    BwdParams ws{};
+    return plan_backward_workspace(d, flags, nullptr, ws).bytes;
 }
 
 uint32_t *backward_route_words(const gf_splat_desc &d, void *workspace, size_t *stride) {
-    BwdWorkspace ws;
-    plan_backward_workspace(d, 0u, workspace, &ws);
+    BwdParams ws{};
+    plan_backward_workspace(d, 0u, workspace, ws);
     *stride = ws.cv_block;
     return route_word(ws.canon);
 }
 
 template <int C, bool PROB>
-static int launch_backward_t(const BwdParams &bp, const BwdWorkspace &ws, bool srt, bool det, int num_sms, cudaStream_t stream) {
+static int launch_backward_t(const BwdParams &bp, const BwdPlan &plan, bool srt, bool det, int num_sms, cudaStream_t stream) {
     const gf_splat_desc &d = bp.d;
     const int B = batch_of(d);
     GF_REQUIRE(B <= 65535, GF_ERR_UNSUPPORTED, "splat backward: batch above 65535");
     // canon words (non-zero = "still canonical") and the voxel->point maps (-1 = empty) in one fill
-    GF_CUDA_TRY(cudaMemsetAsync(bp.canon, 0xFF, ws.cv_bytes, stream));
+    GF_CUDA_TRY(cudaMemsetAsync(bp.canon, 0xFF, plan.cv_bytes, stream));
     const long long want = (static_cast<long long>(d.N) + 255) / 256;
     const int grid0 = static_cast<int>(want < 16ll * num_sms ? (want > 0 ? want : 1) : 16ll * num_sms);
     if (bp.bin_active) {
@@ -418,14 +405,14 @@ static int launch_backward_t(const BwdParams &bp, const BwdWorkspace &ws, bool s
         // the Gaussian-centric chain below finds the flag set and returns.  pack is launched in plain stream order (it
         // starts when everything above has completed); the kernels after it are chained to their predecessor.
         // Deterministic mode: list -> slot plan -> bin (slot stores) -> slot reduce + finish; no accumulator to clear.
-        if (!det) GF_CUDA_TRY(cudaMemsetAsync(ws.sums, 0, ws.sums_bytes, stream));   // accumulated with atomics
+        if (!det) GF_CUDA_TRY(cudaMemsetAsync(bp.sums, 0, plan.sums_bytes, stream));   // accumulated with atomics
         if (PROB) {
             prob_aux_kernel<<<dim3(grid0, B), 256, 0, stream>>>(bp, C);
             GF_CUDA_TRY(cudaGetLastError());
         }
-        int rc = launch_prep(d, bp.in, ws.fwd, 0u, stream, true);
+        int rc = launch_prep(d, bp.in, bp.fwd, 0u, stream, true);
         if (rc != GF_OK) return rc;
-        rc = launch_backward_bin(bp, ws.fwd, ws.sums, det ? &ws.slots : nullptr, stream);
+        rc = launch_backward_bin(bp, det, stream);
         if (rc != GF_OK) return rc;
         // the Gaussian-centric chain is only the fallback now: small grids (they return at once when the points are canonical)
         GF_CUDA_TRY(launch_chained(voxel_map_kernel, dim3(num_sms, B), dim3(256), 0, stream, bp));
@@ -461,33 +448,23 @@ static int launch_backward_t(const BwdParams &bp, const BwdWorkspace &ws, bool s
 
 int launch_backward(const gf_splat_desc &d, const gf_splat_inputs &in, const gf_splat_grads &gr, void *workspace,
                     uint32_t flags, int num_sms, cudaStream_t stream) {
-    BwdWorkspace ws;
-    plan_backward_workspace(d, flags, workspace, &ws);
-    BwdParams bp;
+    BwdParams bp{};
     bp.d = d;
     bp.in = in;
     bp.gr = gr;
+    const BwdPlan plan = plan_backward_workspace(d, flags, workspace, bp);
     const bool srt = in.cov == nullptr;
     if (srt) {   // the pair kernels write the [G,6] gradient of Sigma^-1 into the workspace; srt_grad_kernel maps it on
         bp.d.cov_stride = 6;
-        bp.gr.cov_grad = ws.cov6;
+        bp.gr.cov_grad = bp.cov6;
     }
-    bp.v2p = ws.v2p;
-    bp.big = ws.big;
-    bp.big_ctr = ws.big_ctr;
-    bp.chunk = chunk_voxels(d);
-    bp.canon = ws.canon;
-    bp.aux = ws.aux;
-    bp.cv_block = ws.cv_block;
     bp.bin_active = backward_bin_eligible(bp.d, bp.in, bp.gr) ? 1 : 0;
-    bp.det_cnt = ws.det_cnt;
-    bp.det_part = ws.det_part;
     const bool det = (flags & GF_BWD_DETERMINISTIC) != 0;
     const bool prob = d.variant == GF_SPLAT_PROB;
     return dispatch_classes(d.C, "splat backward", [&](auto cc) {
         constexpr int C = decltype(cc)::value;
-        return prob ? launch_backward_t<C, true>(bp, ws, srt, det, num_sms, stream)
-                    : launch_backward_t<C, false>(bp, ws, srt, det, num_sms, stream);
+        return prob ? launch_backward_t<C, true>(bp, plan, srt, det, num_sms, stream)
+                    : launch_backward_t<C, false>(bp, plan, srt, det, num_sms, stream);
     });
 }
 

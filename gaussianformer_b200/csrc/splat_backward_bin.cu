@@ -17,7 +17,7 @@
 //     nuScenes workload -- a whole warp per Gaussian would spend more on its reduction than on the pairs), read their
 //     pair's point, gradient row and aux terms from shared memory, accumulate the 28 (+1) sums of GaussAcc, reduce them
 //     with a transposing reduction over the eight lanes (28 shuffles for four Gaussians) and add the raw sums to a
-//     [G, 32] accumulator with one atomic per value;
+//     value-major [32, G] accumulator with one atomic per value;
 //   * bin_finish_kernel applies the per-Gaussian linear maps (finish(), splat_bwd_common.cuh) once per Gaussian.
 //
 // The accumulator is zero-filled by the host first.  Summation order across bins is not fixed (fp32 atomics), so two
@@ -45,13 +45,6 @@ struct alignas(64) BinMaps {
     CUtensorMap grad;   // logits_grad as [B*H][W][D*C]
     CUtensorMap pts;    // pts as [B*H or H][W][D*3]
     CUtensorMap aux;    // prob: aux as [B*H][W][D*4]
-};
-
-struct BinParams {
-    SplatWorkspace ws;        // raw records of the pack kernel, boxes and supertile lists
-    float *sums;              // [B, 32, G] raw sums (value-major), zero-filled by the host
-    int nbx;
-    BinSlots det;             // deterministic mode: the slot rows (det.slots == NULL otherwise)
 };
 
 // Bins (kBinX x kBinY x kBinZ voxels) a Gaussian's clipped box overlaps: a rectangle of nb[0] x nb[1] x nb[2] bins from
@@ -144,20 +137,21 @@ __device__ __forceinline__ void check_bin_order(const BwdParams &p, BinSmem<C, P
     }
 }
 
-// DET (deterministic mode): instead of adding the eight lanes' raw sums to the [B, 32, G] accumulator with atomics, the
+// DET (deterministic mode): instead of adding the eight lanes' raw sums to the [32, G] accumulator with atomics, the
 // group stores them to the (Gaussian, bin) pair's own slot row, one 16-byte store per lane.  A pair's sums do not
 // depend on scheduling: the entry's lanes, strides and wide/narrow choice follow from the entry alone, and the shuffle
 // trees are fixed.  With a slot overflow (the route word says so, and the canon flag is already clear) nothing is stored.
+// nbx: bins along x (blockIdx.z = sample * nbx + bin x).
 template <int C, bool PROB, bool DET>
-__device__ __forceinline__ void backward_bin(const BwdParams &pb, const BinParams &bp, const BinMaps &maps) {
+__device__ __forceinline__ void backward_bin(const BwdParams &pb, int nbx, const BinMaps &maps) {
     constexpr int NT = kBinThreads, CP2 = (C + 1) / 2;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     BinSmem<C, PROB> &sm = *reinterpret_cast<BinSmem<C, PROB> *>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int sample = blockIdx.z / bp.nbx;
+    const int sample = blockIdx.z / nbx;
     const BwdParams p = sample_bwd(pb, sample);
     const int H = p.d.H;
-    const int binX0 = (blockIdx.z - sample * bp.nbx) * kBinX, binY0 = blockIdx.y * kBinY, binZ0 = blockIdx.x * kBinZ;
+    const int binX0 = (blockIdx.z - sample * nbx) * kBinX, binY0 = blockIdx.y * kBinY, binZ0 = blockIdx.x * kBinZ;
     if (tid == 0) {
         mbar_init(&sm.bar, 1);
         mbar_fence_init();
@@ -177,7 +171,7 @@ __device__ __forceinline__ void backward_bin(const BwdParams &pb, const BinParam
     }
 
     // ---- candidates: the ascending list of this bin's supertile ------------------------------------------------
-    const SplatWorkspace ws = sample_ws(bp.ws, p.d.G, sample);
+    const SplatWorkspace &ws = p.fwd;
     const bool slot_stores = DET && *p.canon != 0;   // cleared by the slot plan on overflow (or already by a stray point)
     const int s = supertile_of(ws, binX0, binY0);
     const int ncand = ws.counts[s];
@@ -239,7 +233,6 @@ __device__ __forceinline__ void backward_bin(const BwdParams &pb, const BinParam
         __syncthreads();
 
         // ======================= Phase B: eight lanes (or a whole warp) per listed Gaussian ===========
-        float *sums = bp.sums + static_cast<size_t>(sample) * p.d.G * 32;
         const int n_narrow = sm.n_narrow, narrow_tickets = (n_narrow + 3) >> 2;
         const int tickets = narrow_tickets + (nlist - n_narrow);
 #pragma unroll 1
@@ -327,49 +320,45 @@ __device__ __forceinline__ void backward_bin(const BwdParams &pb, const BinParam
                     // slot of (g, this bin): slot_off[g] + the bin's position in the rectangle of bins g's box covers
                     const BoxBins bb(ws.boxes[g]);
                     const int rx = binX0 / kBinX - bb.b0[0], ry = binY0 / kBinY - bb.b0[1], rz = binZ0 / kBinZ - bb.b0[2];
-                    const uint32_t slot = bp.det.slot_off[static_cast<size_t>(sample) * p.d.G + g] +
-                                          static_cast<uint32_t>((rx * bb.nb[1] + ry) * bb.nb[2] + rz);
-                    float4 *row = reinterpret_cast<float4 *>(bp.det.slots + (static_cast<size_t>(sample) * bp.det.budget + slot) * 32);
+                    const uint32_t slot = p.slot_off[g] + static_cast<uint32_t>((rx * bb.nb[1] + ry) * bb.nb[2] + rz);
+                    float4 *row = reinterpret_cast<float4 *>(p.slots + static_cast<size_t>(slot) * 32);
                     row[sub] = make_float4(x[0], x[1], x[2], x[3]);   // values 4*sub .. 4*sub+3 (see group8_transpose_reduce)
                 }
             } else if (have && (!wide || grp == 0)) {
                 const int v0 = ((sub & 4) ? 16 : 0) + ((sub & 2) ? 8 : 0) + ((sub & 1) ? 4 : 0);
 #pragma unroll
                 for (int i = 0; i < 4; ++i)
-                    if (v0 + i < GaussAcc<C, PROB>::kVals) atomicAdd(sums + static_cast<size_t>(v0 + i) * p.d.G + g, x[i]);
+                    if (v0 + i < GaussAcc<C, PROB>::kVals) atomicAdd(p.sums + static_cast<size_t>(v0 + i) * p.d.G + g, x[i]);
             }
         }
     }
 }
 
 template <int C, bool PROB>
-__global__ void __launch_bounds__(kBinThreads, 2) backward_bin_kernel(const BwdParams pb, const BinParams bp,
+__global__ void __launch_bounds__(kBinThreads, 2) backward_bin_kernel(const BwdParams pb, int nbx,
                                                                        const __grid_constant__ BinMaps maps) {
-    backward_bin<C, PROB, false>(pb, bp, maps);
+    backward_bin<C, PROB, false>(pb, nbx, maps);
 }
 
 template <int C, bool PROB>
-__global__ void __launch_bounds__(kBinThreads, 2) backward_bin_slots_kernel(const BwdParams pb, const BinParams bp,
+__global__ void __launch_bounds__(kBinThreads, 2) backward_bin_slots_kernel(const BwdParams pb, int nbx,
                                                                              const __grid_constant__ BinMaps maps) {
-    backward_bin<C, PROB, true>(pb, bp, maps);
+    backward_bin<C, PROB, true>(pb, nbx, maps);
 }
 
 // Deterministic mode, after list_kernel: per sample (one CTA), slot_off[g] = the exclusive prefix over g of the number of
 // bins g's box covers, and the route word: bin route if the total fits the budget, else slot overflow -- which also
 // clears the canon flag, so the bin kernel stores nothing and the Gaussian-centric chain produces the gradients (the
 // hand-over a stray point triggers).
-__global__ void __launch_bounds__(1024) slot_plan_kernel(const BwdParams pb, const BinParams bp) {
+__global__ void __launch_bounds__(1024) slot_plan_kernel(const BwdParams pb) {
     pdl_launch_dependents();
     pdl_wait();   // the boxes of the pack kernel (list_kernel waited for it)
-    const int sample = blockIdx.x;
-    const BwdParams p = sample_bwd(pb, sample);
-    const PackedBox *boxes = sample_ws(bp.ws, p.d.G, sample).boxes;
-    uint32_t *off = bp.det.slot_off + static_cast<size_t>(sample) * p.d.G;
+    const BwdParams p = sample_bwd(pb, blockIdx.x);
     const unsigned long long total = cta_ordered_scan<1024>(
-        p.d.G, [&](int g) { return static_cast<unsigned long long>(BoxBins(boxes[g]).count()); },
-        [&](int g, unsigned long long o) { off[g] = static_cast<uint32_t>(o); });
+        p.d.G, [&](int g) { return static_cast<unsigned long long>(BoxBins(p.fwd.boxes[g]).count()); },
+        [&](int g, unsigned long long o) { p.slot_off[g] = static_cast<uint32_t>(o); });
     if (threadIdx.x == 0) {
-        const bool fits = total <= static_cast<unsigned long long>(bp.det.budget);
+        const bool fits = total <= static_cast<unsigned long long>(p.budget);
         *route_word(p.canon) = fits ? kRouteBin : kRouteSlotOverflow;
         if (!fits) *p.canon = 0;
     }
@@ -384,18 +373,17 @@ constexpr int kWarpSlots = 128;   // Gaussians with more slot rows are summed by
 // row columns; a Gaussian with more than kWarpSlots rows (the whole-grid one covers every bin) is summed the same way by
 // all 256 threads (32 row columns) with a fixed tree over the warps.  The order depends on the row count only.
 template <int C, bool PROB>
-__global__ void __launch_bounds__(256) bin_slot_finish_kernel(const BwdParams pb, const BinParams bp) {
+__global__ void __launch_bounds__(256) bin_slot_finish_kernel(const BwdParams pb) {
     pdl_launch_dependents();
     pdl_wait();
-    const int sample = blockIdx.y;
-    const BwdParams p = sample_bwd(pb, sample);
+    const BwdParams p = sample_bwd(pb, blockIdx.y);
     const bool canon = *p.canon != 0;
     if (blockIdx.x == 0 && threadIdx.x == 0 && !canon && *route_word(p.canon) == kRouteBin) *route_word(p.canon) = kRouteStrayPoints;
     if (!canon) return;
     const int G = p.d.G, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, q = lane & 7;
-    const PackedBox *boxes = sample_ws(bp.ws, G, sample).boxes;
-    const uint32_t *off = bp.det.slot_off + static_cast<size_t>(sample) * G;
-    const float4 *rows = reinterpret_cast<const float4 *>(bp.det.slots + static_cast<size_t>(sample) * bp.det.budget * 32);
+    const PackedBox *boxes = p.fwd.boxes;
+    const uint32_t *off = p.slot_off;
+    const float4 *rows = reinterpret_cast<const float4 *>(p.slots);
     __shared__ int s_wide[8];
     __shared__ float4 s_red[8][8];
     // lane l ends up with value l of the total of quads t (lane j holds quad j & 7)
@@ -451,7 +439,7 @@ __global__ void __launch_bounds__(256) bin_slot_finish_kernel(const BwdParams pb
 // per-Gaussian linear maps of finish() (splat_bwd_common.cuh): d(mean) = -A * sum(w d), d(cov) = -(1/2 | 1) * sum(w d d^T)
 // (+ the determinant terms of the prob variant), d(sem) = opacity * sum(E g) for the base variant.
 template <int C, bool PROB>
-__global__ void __launch_bounds__(128) bin_finish_kernel(const BwdParams pb, const float *sums_all) {
+__global__ void __launch_bounds__(128) bin_finish_kernel(const BwdParams pb) {
     pdl_launch_dependents();
     pdl_wait();
     const BwdParams p = sample_bwd(pb, blockIdx.y);
@@ -459,7 +447,7 @@ __global__ void __launch_bounds__(128) bin_finish_kernel(const BwdParams pb, con
     const int g = blockIdx.x * 128 + threadIdx.x;
     const int G = p.d.G;
     if (g >= G) return;
-    const float *sums = sums_all + static_cast<size_t>(blockIdx.y) * 32 * G + g;
+    const float *sums = p.sums + g;
     float v[32];
 #pragma unroll
     for (int i = 0; i < GaussAcc<C, PROB>::kVals; ++i) v[i] = __ldg(sums + static_cast<size_t>(i) * G);
@@ -532,30 +520,29 @@ bool backward_bin_eligible(const gf_splat_desc &d, const gf_splat_inputs &in, co
 }
 
 template <int C, bool PROB>
-static int launch_bin_t(const BwdParams &bp, const BinParams &np, const BinMaps &maps, cudaStream_t stream) {
+static int launch_bin_t(const BwdParams &bp, bool det, const BinMaps &maps, cudaStream_t stream) {
     const gf_splat_desc &d = bp.d;
     const int B = batch_of(d);
-    const int nzc = (d.D + kBinZ - 1) / kBinZ, nby = (d.W + kBinY - 1) / kBinY;
-    GF_REQUIRE(nby <= 65535 && static_cast<long long>(np.nbx) * B <= 65535, GF_ERR_UNSUPPORTED,
+    const int nzc = (d.D + kBinZ - 1) / kBinZ, nby = (d.W + kBinY - 1) / kBinY, nbx = (d.H + kBinX - 1) / kBinX;
+    GF_REQUIRE(nby <= 65535 && static_cast<long long>(nbx) * B <= 65535, GF_ERR_UNSUPPORTED,
                "splat backward: grid x batch too large for the bin launch");
     const size_t smem = sizeof(BinSmem<C, PROB>);
-    if (np.det.slots) {
-        GF_CUDA_TRY(launch_chained(slot_plan_kernel, dim3(B), dim3(1024), 0, stream, bp, np));
+    if (det) {
+        GF_CUDA_TRY(launch_chained(slot_plan_kernel, dim3(B), dim3(1024), 0, stream, bp));
         GF_CUDA_TRY(cudaFuncSetAttribute(backward_bin_slots_kernel<C, PROB>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-        GF_CUDA_TRY(launch_chained(backward_bin_slots_kernel<C, PROB>, dim3(nzc, nby, np.nbx * B), dim3(kBinThreads), smem, stream, bp, np, maps));
-        GF_CUDA_TRY(launch_chained(bin_slot_finish_kernel<C, PROB>, dim3((d.G + 7) / 8, B), dim3(256), 0, stream, bp, np));
+        GF_CUDA_TRY(launch_chained(backward_bin_slots_kernel<C, PROB>, dim3(nzc, nby, nbx * B), dim3(kBinThreads), smem, stream, bp, nbx, maps));
+        GF_CUDA_TRY(launch_chained(bin_slot_finish_kernel<C, PROB>, dim3((d.G + 7) / 8, B), dim3(256), 0, stream, bp));
         return GF_OK;
     }
     // per call: the attribute is per device, and a process may drive several
     GF_CUDA_TRY(cudaFuncSetAttribute(backward_bin_kernel<C, PROB>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    GF_CUDA_TRY(launch_chained(backward_bin_kernel<C, PROB>, dim3(nzc, nby, np.nbx * B), dim3(kBinThreads), smem, stream, bp, np, maps));
-    const float *sums = np.sums;
-    GF_CUDA_TRY(launch_chained(bin_finish_kernel<C, PROB>, dim3((d.G + 127) / 128, B), dim3(128), 0, stream, bp, sums));
+    GF_CUDA_TRY(launch_chained(backward_bin_kernel<C, PROB>, dim3(nzc, nby, nbx * B), dim3(kBinThreads), smem, stream, bp, nbx, maps));
+    GF_CUDA_TRY(launch_chained(bin_finish_kernel<C, PROB>, dim3((d.G + 127) / 128, B), dim3(128), 0, stream, bp));
     return GF_OK;
 }
 
-// bp: the launch parameters of the backward (batch-level pointers); fws: the supertile lists built for this call
-int launch_backward_bin(const BwdParams &bp, const SplatWorkspace &fws, float *sums, const BinSlots *slots, cudaStream_t stream) {
+// bp: the launch parameters of the backward (batch-level pointers), with the supertile lists built for this call
+int launch_backward_bin(const BwdParams &bp, bool det, cudaStream_t stream) {
     const gf_splat_desc &d = bp.d;
     const long long B = batch_of(d);
     BinMaps maps;
@@ -564,11 +551,10 @@ int launch_backward_bin(const BwdParams &bp, const SplatWorkspace &fws, float *s
     if (d.variant == GF_SPLAT_PROB) ok = ok && make_map(&maps.aux, bp.aux, B * d.H, d.W, d.D * 4, kBinZ * 4);
     else maps.aux = maps.pts;
     GF_REQUIRE(ok, GF_ERR_CUDA, "splat backward: cuTensorMapEncodeTiled failed");
-    const BinParams np{fws, sums, (d.H + kBinX - 1) / kBinX, slots ? *slots : BinSlots{nullptr, nullptr, 0}};
     const bool prob = d.variant == GF_SPLAT_PROB;
     return dispatch_classes(d.C, "splat backward", [&](auto cc) {
         constexpr int C = decltype(cc)::value;
-        return prob ? launch_bin_t<C, true>(bp, np, maps, stream) : launch_bin_t<C, false>(bp, np, maps, stream);
+        return prob ? launch_bin_t<C, true>(bp, det, maps, stream) : launch_bin_t<C, false>(bp, det, maps, stream);
     });
 }
 

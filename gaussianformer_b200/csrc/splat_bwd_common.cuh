@@ -11,33 +11,53 @@ constexpr int kBigBox = 2048;
 constexpr int bwd_threads(bool prob) { return prob ? 128 : 256; }
 constexpr int bwd_ctas(bool prob) { return prob ? 3 : 2; }
 
+// Deterministic mode: the big kernel's grid per sample.  A constant, so that the (CTA, segment) split of the queue, and
+// with it the summation order, depends on the inputs only (not on the SM count or the batch size).
+constexpr int kDetBigCtas = 256;
+
+// Launch parameters of every backward kernel: the call's desc and tensors, and the backward workspace.
+//
+// The workspace block is the one description of the workspace: only plan_backward_workspace (splat_backward.cu) sets
+// it, kernels receive it whole and narrow it to one sample with sample_bwd.  Every pointer in it addresses B
+// consecutive per-sample blocks, shaped as given; the deterministic-only regions (GF_BWD_DETERMINISTIC) are carved
+// behind all others, so the layout without the flag is unchanged, and are NULL without it.
+// The block stays flat and its first ten fields keep their offsets behind gr: the Gaussian-centric kernels run at
+// their register cap, and ptxas allocates several of them differently (some with almost three times the spill
+// traffic) when these fields move or sit in a struct of their own.  Check -Xptxas -v before reordering.
 struct BwdParams {
     gf_splat_desc d;
     gf_splat_inputs in;
     gf_splat_grads gr;
-    int32_t *v2p;      // [H*W*D]
-    uint2 *big;        // [G] queue of the boxes larger than kBigBox: (Gaussian, first chunk), ascending in both
-    unsigned long long *big_ctr;   // queue length << 40 | chunks queued (one atomic keeps the two in step)
-    int chunk;         // box voxels per chunk
-    int32_t *canon;    // non-zero after voxel_map_kernel iff N == H*W*D and point n sits in voxel n for all n
-    float4 *aux;       // [N] prob only: per-point terms that do not depend on the Gaussian
+    // ---- workspace
+    int32_t *v2p;      // [H*W*D] per canon block: voxel -> largest point index in it, -1 for none
+    uint2 *big;        // [B,G] queue of the boxes larger than kBigBox: (Gaussian, first chunk), ascending in both
+    unsigned long long *big_ctr;   // [B] queue length << 40 | chunks queued (one atomic keeps the two in step)
+    int chunk;         // box voxels per chunk, the unit of big and big_ctr
+    // Per sample, cv_block bytes apart: the canon word (256 bytes, filled with 0xFF per call) directly in front of the
+    // voxel -> point map, so that one memset covers all of them.  Non-zero after voxel_map_kernel iff N == H*W*D and
+    // point n sits in voxel n for all n; word 1 is the route word (route_word).
+    int32_t *canon;
+    float4 *aux;       // [B,N] prob only: per-point terms that do not depend on the Gaussian
     size_t cv_block;   // bytes between the (canon, v2p) blocks of consecutive samples
+    long long budget;  // deterministic: slot rows per sample
+    uint32_t *det_cnt; // deterministic: [B,G] chunks of each Gaussian's box when it is queued for the big kernel, else 0
+    float *det_part;   // deterministic: [B,G + kDetBigCtas,32] raw sums of the big kernel, one row per (CTA, entry) segment
+    float *cov6;       // [B,G,6] gradient of Sigma^-1 when the caller passed scales + rotations instead of cov
+    SplatWorkspace fwd;   // records, boxes and supertile lists for the bin-centric kernel
+    float *sums;       // [B,32,G] raw sums of the bin-centric kernel (value-major), zero-filled by the host
+    uint32_t *slot_off;   // deterministic: [B,G] first slot row of Gaussian g in the bin route
+    float *slots;      // deterministic: [B,budget,32] raw sums of the bin route, one row per (Gaussian, bin) pair
+    // ----
     int bin_active;    // the bin-centric kernel (splat_backward_bin.cu) serves this call when the points are canonical
-    // deterministic mode only (GF_BWD_DETERMINISTIC), NULL otherwise
-    uint32_t *det_cnt; // [G] chunks of each Gaussian's box when it is queued for the big kernel, else 0
-    float *det_part;   // [G + kDetBigCtas][32] raw sums of the big kernel, one row per (CTA, queue entry) segment
 };
-
-// Deterministic mode: the big kernel's grid per sample.  A constant, so that the (CTA, segment) split of the queue, and
-// with it the summation order, depends on the inputs only (not on the SM count or the batch size).
-constexpr int kDetBigCtas = 256;
 
 // Word 1 of a sample's canon block (the 256 bytes in front of its voxel -> point map, filled with 0xFF per call): which
 // route produced the gradients of a deterministic backward (GF_DEBUG_ROUTE_*, include/gf_b200_debug.h).
 __host__ __device__ inline uint32_t *route_word(int32_t *canon) { return reinterpret_cast<uint32_t *>(canon) + 1; }
 constexpr uint32_t kRouteBin = 0, kRouteSlotOverflow = 1, kRouteStrayPoints = 2, kRouteGaussian = 3;
 
-// The launch parameters narrowed to sample b of the batch (the kernels run with blockIdx.y = sample).
+// The launch parameters narrowed to sample b of the batch: its tensors and its blocks of the workspace.  The only code
+// that computes per-sample offsets into the backward workspace.
 __device__ __forceinline__ BwdParams sample_bwd(const BwdParams &p, int b) {
     BwdParams q = p;
     q.in = sample_inputs(p.d, p.in, b);
@@ -47,6 +67,11 @@ __device__ __forceinline__ BwdParams sample_bwd(const BwdParams &p, int b) {
     q.big = p.big + static_cast<size_t>(b) * p.d.G;
     q.big_ctr = p.big_ctr + b;
     q.aux = adv(p.aux, static_cast<long long>(b) * p.d.N);
+    q.cov6 = p.cov6 + static_cast<size_t>(b) * p.d.G * 6;
+    q.fwd = sample_ws(p.fwd, p.d.G, b);
+    q.sums = p.sums + static_cast<size_t>(b) * 32 * p.d.G;
+    q.slot_off = adv(p.slot_off, static_cast<long long>(b) * p.d.G);
+    q.slots = adv(p.slots, static_cast<long long>(b) * p.budget * 32);
     q.det_cnt = adv(p.det_cnt, static_cast<long long>(b) * p.d.G);
     q.det_part = adv(p.det_part, static_cast<long long>(b) * (p.d.G + kDetBigCtas) * 32);
     return q;

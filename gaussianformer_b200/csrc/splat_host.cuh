@@ -30,14 +30,6 @@ int launch_render(const gf_splat_desc &d, const gf_splat_inputs &in, const gf_sp
                   const SplatWorkspace &ws, bool tile_path, int num_sms, cudaStream_t stream);
 int render_ctas_per_sample(const gf_splat_desc &d);
 
-// The deterministic bin route's slots (GF_BWD_DETERMINISTIC): one row of 32 fp32 raw sums per (Gaussian, bin) pair,
-// the rows of Gaussian g starting at slot_off[g].
-struct BinSlots {
-    float *slots;        // [B, budget, 32]
-    uint32_t *slot_off;  // [B, G]
-    long long budget;    // slots per sample
-};
-
 // splat_backward.cu
 size_t backward_workspace_bytes(const gf_splat_desc &d, uint32_t flags);
 int launch_backward(const gf_splat_desc &d, const gf_splat_inputs &in, const gf_splat_grads &gr, void *workspace,
@@ -47,8 +39,8 @@ uint32_t *backward_route_words(const gf_splat_desc &d, void *workspace, size_t *
 
 // splat_backward_bin.cu
 bool backward_bin_eligible(const gf_splat_desc &d, const gf_splat_inputs &in, const gf_splat_grads &gr);
-// slots: NULL for the atomic accumulation into sums, else the deterministic slot route
-int launch_backward_bin(const BwdParams &bp, const SplatWorkspace &fws, float *sums, const BinSlots *slots, cudaStream_t stream);
+// det: the deterministic slot route (bp.slots) instead of the atomic accumulation into bp.sums
+int launch_backward_bin(const BwdParams &bp, bool det, cudaStream_t stream);
 
 // cabi.cu: events recorded around the render kernel when both are set (gf_debug_set_render_events)
 extern thread_local cudaEvent_t g_ev_before, g_ev_after;
