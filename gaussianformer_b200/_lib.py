@@ -39,6 +39,7 @@ EXPORTS = (
     "gf_daf_format_ex", "gf_splat_backward_workspace_bytes_ex", "gf_splat_backward_ex",
     "gf_daf_backward_workspace_bytes", "gf_daf_backward_ex2", "gf_daf_fused_backward_workspace_bytes",
     "gf_daf_fused_backward_ex2", "gf_daf_project", "gf_daf_project_backward",
+    "gf_daf_anchor_key_points", "gf_daf_anchor_key_points_backward",
 )
 
 
@@ -83,6 +84,12 @@ DAF_MAX_LEVELS = 8
 class DafFormatDesc(Structure):
     _fields_ = [("batch_cams", c_int32), ("num_embeds", c_int32), ("num_scale", c_int32),
                 ("hw", c_int32 * DAF_MAX_LEVELS)]
+
+
+class DafKpsDesc(Structure):
+    _fields_ = [("batch", c_int32), ("num_anchors", c_int32), ("anchor_dim", c_int32), ("num_fixed", c_int32),
+                ("num_learnable", c_int32), ("lo", c_float * 3), ("extent", c_float * 3), ("scale_lo", c_float),
+                ("scale_extent", c_float), ("learnable_fixed_scale", c_float)]
 
 
 class GfError(RuntimeError):
@@ -144,6 +151,8 @@ def lib():
         L.gf_debug_daf_plan.argtypes = [c_int32]
         L.gf_daf_project.argtypes = [c_int32, c_int32, c_int32] + [c_void_p] * 6
         L.gf_daf_project_backward.argtypes = [c_int32, c_int32, c_int32] + [c_void_p] * 6
+        L.gf_daf_anchor_key_points.argtypes = [POINTER(DafKpsDesc)] + [c_void_p] * 5
+        L.gf_daf_anchor_key_points_backward.argtypes = [POINTER(DafKpsDesc)] + [c_void_p] * 7
         if L.gf_abi_version() != 2:
             raise ImportError("libgf_b200.so: ABI version mismatch")
         _lib = L

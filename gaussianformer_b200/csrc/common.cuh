@@ -356,15 +356,44 @@ __device__ __forceinline__ gf_splat_grads sample_grads(const gf_splat_desc &d, c
     return o;
 }
 
+// The scalar-type overloads the quaternion maps below are written with (float: the splat, double: the key-point
+// generator of daf_anchor.cu).
+__device__ __forceinline__ float q_sqrt(float v) { return sqrtf(v); }
+__device__ __forceinline__ double q_sqrt(double v) { return sqrt(v); }
+__device__ __forceinline__ float q_max(float a, float b) { return fmaxf(a, b); }
+__device__ __forceinline__ double q_max(double a, double b) { return fmax(a, b); }
+__device__ __forceinline__ float q_div(float a, float b) { return __fdiv_rn(a, b); }
+__device__ __forceinline__ double q_div(double a, double b) { return __ddiv_rn(a, b); }
+
 // Rotation matrix of the NORMALISED quaternion (w,x,y,z) -- get_rotation_matrix, model/utils/utils.py:20-66
-// (F.normalize: q / max(|q|, 1e-12)).  R[k][l], row-major.
-__device__ __forceinline__ void quat_rotation(const float q[4], float R[3][3], float &inv_norm) {
-    const float n = sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
-    inv_norm = __fdiv_rn(1.f, fmaxf(n, 1e-12f));
-    const float w = q[0] * inv_norm, x = q[1] * inv_norm, y = q[2] * inv_norm, z = q[3] * inv_norm;
-    R[0][0] = w * w + x * x - y * y - z * z; R[0][1] = 2.f * (x * y - w * z);         R[0][2] = 2.f * (x * z + w * y);
-    R[1][0] = 2.f * (x * y + w * z);         R[1][1] = w * w - x * x + y * y - z * z; R[1][2] = 2.f * (y * z - w * x);
-    R[2][0] = 2.f * (x * z - w * y);         R[2][1] = 2.f * (y * z + w * x);         R[2][2] = w * w - x * x - y * y + z * z;
+// (F.normalize: q / max(|q|, 1e-12), the epsilon as an fp32 tensor holds it).  R[k][l], row-major.  Returns |q|.
+template <class T>
+__device__ __forceinline__ T quat_rotation(const T q[4], T R[3][3], T &inv_norm) {
+    const T n = q_sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+    inv_norm = q_div(T(1), q_max(n, static_cast<T>(1e-12f)));
+    const T w = q[0] * inv_norm, x = q[1] * inv_norm, y = q[2] * inv_norm, z = q[3] * inv_norm;
+    R[0][0] = w * w + x * x - y * y - z * z; R[0][1] = T(2) * (x * y - w * z);         R[0][2] = T(2) * (x * z + w * y);
+    R[1][0] = T(2) * (x * y + w * z);         R[1][1] = w * w - x * x + y * y - z * z; R[1][2] = T(2) * (y * z - w * x);
+    R[2][0] = T(2) * (x * z - w * y);         R[2][1] = T(2) * (y * z + w * x);         R[2][2] = w * w - x * x - y * y + z * z;
+    return n;
+}
+
+// The gradient of quat_rotation: dq (w.r.t. the UN-normalised q) from M = dL/dR, through the quaternion -> matrix map and
+// F.normalize.  inv_norm is quat_rotation's.  below_eps: |q| < 1e-12, where F.normalize divides by the constant epsilon,
+// so the gradient is M's pulled back and scaled, without the projection onto the sphere's tangent.
+template <class T>
+__device__ __forceinline__ void quat_rotation_backward(const T q[4], T inv_norm, const T M[3][3], T dq[4],
+                                                       bool below_eps) {
+    const T w = q[0] * inv_norm, x = q[1] * inv_norm, y = q[2] * inv_norm, z = q[3] * inv_norm;
+    const T gw = T(2) * (w * (M[0][0] + M[1][1] + M[2][2]) - z * M[0][1] + y * M[0][2] + z * M[1][0] - x * M[1][2] - y * M[2][0] + x * M[2][1]);
+    const T gx = T(2) * (x * (M[0][0] - M[1][1] - M[2][2]) + y * M[0][1] + z * M[0][2] + y * M[1][0] - w * M[1][2] + z * M[2][0] + w * M[2][1]);
+    const T gy = T(2) * (y * (-M[0][0] + M[1][1] - M[2][2]) + x * M[0][1] + w * M[0][2] + x * M[1][0] + z * M[1][2] - w * M[2][0] + z * M[2][1]);
+    const T gz = T(2) * (z * (-M[0][0] - M[1][1] + M[2][2]) - w * M[0][1] + x * M[0][2] + w * M[1][0] + y * M[1][2] + x * M[2][0] + y * M[2][1]);
+    const T dot = below_eps ? T(0) : w * gw + x * gx + y * gy + z * gz;
+    dq[0] = inv_norm * (gw - w * dot);
+    dq[1] = inv_norm * (gx - x * dot);
+    dq[2] = inv_norm * (gy - y * dot);
+    dq[3] = inv_norm * (gz - z * dot);
 }
 
 // Sigma^-1 = R^T diag(1/s^2) R as (xx,yy,zz,xy,yz,xz): the closed form of GaussianHead.prepare_gaussian_args'

@@ -309,16 +309,11 @@ __global__ void __launch_bounds__(128) srt_grad_kernel(const BwdParams pb) {
 #pragma unroll
         for (int l = 0; l < 3; ++l) M[k][l] = Dk * t[l];
     }
-    const float w = q[0] * inv_norm, x = q[1] * inv_norm, y = q[2] * inv_norm, z = q[3] * inv_norm;
-    const float gw = 2.f * (w * (M[0][0] + M[1][1] + M[2][2]) - z * M[0][1] + y * M[0][2] + z * M[1][0] - x * M[1][2] - y * M[2][0] + x * M[2][1]);
-    const float gx = 2.f * (x * (M[0][0] - M[1][1] - M[2][2]) + y * M[0][1] + z * M[0][2] + y * M[1][0] - w * M[1][2] + z * M[2][0] + w * M[2][1]);
-    const float gy = 2.f * (y * (-M[0][0] + M[1][1] - M[2][2]) + x * M[0][1] + w * M[0][2] + x * M[1][0] + z * M[1][2] - w * M[2][0] + z * M[2][1]);
-    const float gz = 2.f * (z * (-M[0][0] - M[1][1] + M[2][2]) - w * M[0][1] + x * M[0][2] + w * M[1][0] + y * M[1][2] + x * M[2][0] + y * M[2][1]);
-    const float dot = w * gw + x * gx + y * gy + z * gz;
-    p.gr.rotations_grad[4 * g] = inv_norm * (gw - w * dot);
-    p.gr.rotations_grad[4 * g + 1] = inv_norm * (gx - x * dot);
-    p.gr.rotations_grad[4 * g + 2] = inv_norm * (gy - y * dot);
-    p.gr.rotations_grad[4 * g + 3] = inv_norm * (gz - z * dot);
+    // every quaternion takes the tangent projection here, as it always has: the splat's rotations are never near 0
+    float dq[4];
+    quat_rotation_backward(q, inv_norm, M, dq, false);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) p.gr.rotations_grad[4 * g + i] = dq[i];
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -291,6 +291,83 @@ def make_daf_kp_inputs(num_anchor=25600, num_pts=9, batch=1, num_cams=6, embed_d
     return feature_maps, kps.contiguous(), proj, wh, logits, weight_mask
 
 
+# The key-point generator of both shipped families: fix_scale of config/_base_/model.py:88-96; GaussianFormer-1
+# config/nuscenes_gs25600_solid.py:69-70,124-131, GaussianFormer-2 config/prob/nuscenes_gs6400.py:87-88,173-181.
+ANCHOR_FIX_SCALE = ((0.0, 0.0, 0.0), (0.45, 0.0, 0.0), (-0.45, 0.0, 0.0), (0.0, 0.45, 0.0), (0.0, -0.45, 0.0),
+                    (0.0, 0.0, 0.45), (0.0, 0.0, -0.45))
+ANCHOR_KP_CONFIGS = {
+    "gs25600_solid": dict(num_anchor=25600, num_learnable=2, learnable_fixed_scale=1.0,
+                          pc_range=(-50.0, -50.0, -5.0, 50.0, 50.0, 3.0), scale_range=(0.08, 0.64)),
+    "prob_gs6400": dict(num_anchor=6400, num_learnable=6, learnable_fixed_scale=6.0,
+                        pc_range=(-50.0, -50.0, -5.0, 50.0, 50.0, 3.0), scale_range=(0.01, 3.2)),
+}
+ANCHOR_DIM = 28          # xyz, scale, rotation, opacity, semantics
+
+
+def _key_points_fp64(anchor, logits, cfg):
+    """SparseGaussian3DKeyPointsGenerator.forward in fp64 (for the margin test of make_anchor_kp_inputs only)."""
+    a = anchor.double()
+    sig = lambda v: torch.sigmoid(v.clamp(-9.21, 9.21))                                 # noqa: E731
+    lo, hi = torch.tensor(cfg["pc_range"][:3]).double(), torch.tensor(cfg["pc_range"][3:]).double()
+    s0, s1 = cfg["scale_range"]
+    xyz = lo + (hi - lo) * sig(a[..., 0:3])
+    gs = s0 + (s1 - s0) * sig(a[..., 3:6])
+    B, A = a.shape[:2]
+    s = torch.tensor(ANCHOR_FIX_SCALE, dtype=torch.float64).expand(B, A, -1, -1)
+    s = torch.cat([s, (sig(logits.double()) - 0.5) * cfg["learnable_fixed_scale"]], 2)
+    R = quat_to_rotmat(a[..., 6:10])
+    return torch.einsum("bajk,bapj->bapk", R, s * gs[:, :, None]) + xyz[:, :, None]           # R^T v + xyz
+
+
+def make_anchor_kp_inputs(config="gs25600_solid", batch=1, num_anchor=None, embed_dims=128, seed=0, margin=False,
+                          num_cams=6, levels=DAF_LEVELS_1600x864, image_wh=(1600.0, 864.0)):
+    """Inputs of ``ops.anchor_key_points`` / ``ops.SparseGaussian3DKeyPointsGenerator`` for one of
+    ``ANCHOR_KP_CONFIGS``: anchors ``[B, A, 28]`` (xyz logits of a uniform position in pc_range, N(0, 1) scale logits,
+    an un-normalised N(0, 1) quaternion, N(0, 1) opacity and semantics), an ``instance_feature`` ``[B, A, embed_dims]``,
+    a seeded ``learnable_fc`` (``weight``, ``bias``, xavier-uniform) and its output ``logits`` ``[B, A, Kl, 3]``
+    (fp32, on the CPU), plus the camera rig of ``make_daf_kp_inputs`` (``projection_mat``, ``image_wh``).
+
+    ``margin=True`` keeps every anchor and learnable logit at least 1e-3 from +-9.21 (instance features are re-drawn
+    for the learnable ones), and re-draws every anchor one of whose key points ``_near_a_boundary`` flags, so that an
+    fp32 PyTorch generator and projection decide every gate, mask and bilinear cell as the fp64 ones do.  Returns a
+    dict with those tensors and the generator's ``fix_scale``, ``pc_range``, ``scale_range``,
+    ``learnable_fixed_scale`` and ``num_learnable``."""
+    cfg = ANCHOR_KP_CONFIGS[config]
+    A = cfg["num_anchor"] if num_anchor is None else num_anchor
+    Kl = cfg["num_learnable"]
+    gen = torch.Generator().manual_seed(seed)
+
+    def draw_anchors(n):
+        u = torch.rand(n, 3, generator=gen) * 0.96 + 0.02
+        return torch.cat([torch.log(u / (1 - u)), torch.randn(n, ANCHOR_DIM - 3, generator=gen)], -1)
+
+    anchor = draw_anchors(batch * A).reshape(batch, A, ANCHOR_DIM)
+    feat = torch.randn(batch, A, embed_dims, generator=gen)
+    bound = math.sqrt(6.0 / (embed_dims + 3 * Kl))
+    weight = (torch.rand(3 * Kl, embed_dims, generator=gen) * 2 - 1) * bound
+    bias = (torch.rand(3 * Kl, generator=gen) * 2 - 1) * 0.1
+    logits = lambda: (feat @ weight.T + bias).reshape(batch, A, Kl, 3)                  # noqa: E731
+    proj = camera_rig(num_cams, image_wh)[None].repeat(batch, 1, 1, 1).contiguous()
+    wh = torch.tensor(image_wh, dtype=torch.float32).repeat(batch, num_cams, 1).contiguous()
+    if margin:
+        near = lambda v: ((v.abs() - 9.21).abs() < 1e-3)                                  # noqa: E731
+        for _ in range(100):
+            bad_f = near(logits()).flatten(2).any(-1)
+            bad_a = near(anchor[..., :6]).any(-1) | _near_a_boundary(
+                _key_points_fp64(anchor, logits(), cfg).float(), proj, wh, levels).any(-1)
+            if not (bad_f.any() or bad_a.any()):
+                break
+            feat[bad_f] = torch.randn(int(bad_f.sum()), embed_dims, generator=gen)
+            anchor[bad_a] = draw_anchors(int(bad_a.sum()))
+        else:
+            raise RuntimeError("make_anchor_kp_inputs: anchors near a boundary after 100 re-draws")
+    return dict(anchor=anchor.contiguous(), instance_feature=feat.contiguous(), weight=weight, bias=bias,
+                logits=logits().contiguous(), projection_mat=proj, image_wh=wh,
+                fix_scale=torch.tensor(ANCHOR_FIX_SCALE), pc_range=list(cfg["pc_range"]),
+                scale_range=list(cfg["scale_range"]), learnable_fixed_scale=cfg["learnable_fixed_scale"],
+                num_learnable=Kl)
+
+
 def reference_fused_composition(daf_apply, feat, shape, start, loc, logits, point_mask=None, weight_mask=None):
     """``deformable_module.py:213-228`` + ``:242`` in PyTorch around an op call ``daf_apply`` — what the fused entry
     point replaces (used by the tests and by bench.py to time the unfused route on the same GPU)."""

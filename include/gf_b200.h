@@ -366,6 +366,48 @@ int gf_daf_project_backward(int32_t batch, int32_t num_pts, int32_t num_cams, co
                             const float *projection_mat, const float *image_wh, const float *grad_loc,
                             float *grad_key_points, gf_stream_t stream);
 
+/* ---- key points of Gaussian anchors: SparseGaussian3DKeyPointsGenerator.forward
+ * (model/encoder/gaussian_encoder/deformable_module.py:51-90), the stage in front of gf_daf_project.  For anchor row
+ * x = anchor[b, a, :] (anchor_dim >= 10 columns: xyz logits, scale logits, quaternion (w, x, y, z), then anything) and
+ * key point k (the num_fixed fixed points first, then the num_learnable learnable ones):
+ *
+ *   sig(v)  = 1 / (1 + exp(-clamp(v, -9.21f, 9.21f)))                                    safe_sigmoid
+ *   xyz     = lo + extent * sig(x[0:3])
+ *   gs      = scale_lo + scale_extent * sig(x[3:6])
+ *   s_k     = fix_scale[k]                                                               k <  num_fixed
+ *           = (sig(learnable_logits[b, a, k - num_fixed]) - 0.5) * learnable_fixed_scale   k >= num_fixed
+ *   key_points[b, a, k] = R^T (s_k * gs) + xyz,   R = get_rotation_matrix(x[6:10]) (model/utils/utils.py:20-69,
+ *                                                 F.normalize with epsilon (double)1e-12f first)
+ *
+ * in fp64 from the fp32 inputs, each output rounded to fp32 once.  The descriptor's floats are the fp32 values the
+ * reference's fp32 tensors multiply by: lo = pc_range[0:3], extent = float(pc_range[3:6] - pc_range[0:3]),
+ * scale_lo = scale_range[0], scale_extent = float(scale_range[1] - scale_range[0]).
+ *
+ * anchor [B, A, anchor_dim], fix_scale [num_fixed, 3], learnable_logits [B, A, num_learnable, 3] (the pre-sigmoid
+ * learnable_fc output; NULL when num_learnable == 0), key_points [B, A, num_fixed + num_learnable, 3], fully
+ * overwritten.
+ *
+ * gf_daf_anchor_key_points_backward: given grad_key_points [B, A, K, 3], fully overwrites grad_anchor
+ * [B, A, anchor_dim] (columns 10 and up are 0) and grad_learnable [B, A, num_learnable, 3] (the gradient of the
+ * pre-sigmoid logits; may be NULL when num_learnable == 0).  One thread per anchor sums over k in ascending order in
+ * fp64 without atomics, so the gradients are bit-reproducible.  The clamps pass the gradient where
+ * -9.21f <= v <= 9.21f, bounds included (torch.clamp's backward), and block it elsewhere.
+ *
+ * Both need no workspace and do not synchronise.  A NULL desc, negative sizes, anchor_dim < 10, no key points for
+ * non-empty work and NULL pointers for non-empty work are GF_ERR_INVALID_ARG; B * A * K >= 2^31 or
+ * B * A * anchor_dim >= 2^31 is GF_ERR_UNSUPPORTED; all before any CUDA call. */
+typedef struct gf_daf_kps_desc {
+    int32_t batch, num_anchors, anchor_dim, num_fixed, num_learnable;
+    float lo[3], extent[3], scale_lo, scale_extent, learnable_fixed_scale;
+} gf_daf_kps_desc;
+
+int gf_daf_anchor_key_points(const gf_daf_kps_desc *desc, const float *anchor, const float *fix_scale,
+                             const float *learnable_logits, float *key_points, gf_stream_t stream);
+
+int gf_daf_anchor_key_points_backward(const gf_daf_kps_desc *desc, const float *anchor, const float *fix_scale,
+                                      const float *learnable_logits, const float *grad_key_points,
+                                      float *grad_anchor, float *grad_learnable, gf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
