@@ -62,9 +62,10 @@ def test_shared_points_and_forward_on_grid_batch():
 @pytest.mark.parametrize("cfg", ["tiny", "tiny_prob"])
 def test_in_kernel_inverse_covariance_and_its_backward(cfg):
     """forward_from_srt: Sigma^-1 = R^T diag(1/s^2) R inside the pack kernel; backward: d/dscales, d/drotations from the
-    srt kernel.  Reference route: the reference's CPU inverse for the values (gaussian_head.py:111-119) and PyTorch
-    autograd through the closed form for the gradients."""
-    from gaussianformer_b200.splat import inverse_covariance_from_srt
+    srt kernel.  Values: against the reference's CPU inverse (gaussian_head.py:111-119) fed through the standard entry
+    point.  Gradients of all five leaves: every sample against the fp64 chain of tests/srt_oracle.py with
+    helpers.assert_grad_parity (srt_oracle.check_grads)."""
+    import srt_oracle as so
     from gaussianformer_b200.synthetic import inverse_covariance
     kw, inps, cat, variant = _batch_of(cfg, (41, 42), True)
     B, G = cat["means"].shape[:2]
@@ -75,23 +76,23 @@ def test_in_kernel_inverse_covariance_and_its_backward(cfg):
     # values: against the reference's numerical inverse fed through the standard entry point
     ref_cov = inverse_covariance(cat["scales"], rots).float().cuda()
     out_ref = m(t["pts"], t["means"], t["opa"], t["sem"], t["scales"], ref_cov)
-    s1 = cat["scales"].cuda().requires_grad_(True); r1 = rots.cuda().requires_grad_(True)
-    mu1 = t["means"].clone().requires_grad_(True)
-    out = m.forward_from_srt(t["pts"], mu1, t["opa"], t["sem"], s1, r1)
+    leaves = {k: t[k].clone().requires_grad_(True) for k in ("means", "opa", "sem", "scales")}
+    leaves["rotations"] = rots.cuda().requires_grad_(True)
+    out = m.forward_from_srt(t["pts"], leaves["means"], leaves["opa"], leaves["sem"], leaves["scales"], leaves["rotations"])
     first = out if variant == "base" else out[0]
     first_ref = out_ref if variant == "base" else out_ref[0]
     h.assert_close(first.detach().cpu().numpy(), first_ref.cpu().numpy(), rtol=1e-3, atol=1e-4, what="logits from s, r")
-    # gradients: autograd through the PyTorch closed form + the standard op
-    s2 = cat["scales"].cuda().requires_grad_(True); r2 = rots.cuda().requires_grad_(True)
-    mu2 = t["means"].clone().requires_grad_(True)
-    out2 = m(t["pts"], mu2, t["opa"], t["sem"], s2.detach(), inverse_covariance_from_srt(s2, r2))
-    outs, outs2 = ((out,), (out2,)) if variant == "base" else (tuple(out), tuple(out2))
-    gs = [torch.randn(o.shape, generator=gen).cuda() for o in outs]
-    torch.autograd.backward(list(outs), gs)
-    torch.autograd.backward(list(outs2), gs)
-    for name, a, b in (("scales", s1.grad, s2.grad), ("rotations", r1.grad, r2.grad), ("means", mu1.grad, mu2.grad)):
-        ref = b.cpu().numpy()
-        h.assert_close(a.cpu().numpy(), ref, rtol=2e-3, atol=2e-4 * max(1.0, float(np.abs(ref).max())), what=f"{cfg} grad {name}")
+    # gradients: against the fp64 chain, per sample
+    outs = (out,) if variant == "base" else tuple(out)
+    gs = [torch.randn(o.shape, generator=gen) for o in outs]
+    torch.autograd.backward(list(outs), [x.cuda() for x in gs])
+    for b, inp in enumerate(inps):
+        mine_out = [o[b].detach().cpu().numpy() for o in outs]
+        chains = so.srt_chains(kw, inp, inp["scales"][0], rots[b], variant, tuple(x[b].numpy() for x in gs),
+                               op_outputs=mine_out[:2])
+        so.check_grads({k: v.grad[b].cpu().numpy() for k, v in leaves.items()}, chains[0][1], chains[1][1],
+                       f"{cfg} sample {b}")
+    r1, s1 = leaves["rotations"], leaves["scales"]
     assert float(r1.grad.abs().max()) > 0 and torch.isfinite(s1.grad).all()
     # the gradient of an un-normalised quaternion is orthogonal to it (F.normalize)
     dots = (r1.grad * r1.detach()).sum(-1).abs().max()

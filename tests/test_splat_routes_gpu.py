@@ -238,35 +238,17 @@ def test_forward_on_grid_batch_vs_oracle(variant):
 @pytest.mark.parametrize("variant", VARIANTS)
 def test_forward_from_srt_generic_route(variant):
     """forward_from_srt on permuted points: the Gaussian-centric chain writes the gradient of Sigma^-1 (stride 6) and
-    srt_grad_kernel maps it to scales and rotations.  Reference: the fp64 oracle's gradient of Sigma^-1 pushed through
-    the closed form R^T diag(1/s^2) R in float64 by autograd."""
-    from gaussianformer_b200.splat import inverse_covariance_from_srt
+    srt_grad_kernel maps it to scales and rotations.  Reference: the fp64 chain of tests/srt_oracle.py (Sigma^-1, the
+    oracle and autograd through the closed form R^T diag(1/s^2) R in float64), with the gates of
+    test_splat_srt_gpu.check_srt; under use_deterministic_algorithms the deterministic backward."""
+    import test_splat_srt_gpu as srt
     kw, inp = _case(variant)
     G = inp["means"].shape[1]
     gen = torch.Generator().manual_seed(23)
     rots = torch.randn(1, G, 4, generator=gen) * 1.5
     perm = torch.randperm(inp["pts"].shape[1], generator=gen)
-    cov = inverse_covariance_from_srt(inp["scales"].double(), rots.double()).float()
-    inp = dict(inp, pts=inp["pts"][:, perm].contiguous(), cov=cov)
-    _assert_big_box(kw, inp, variant)
-    m = h.make_module(kw, variant)
-    t = h.to_dev(inp)
-    s_d = inp["scales"].cuda().requires_grad_(True)
-    r_d = rots.cuda().requires_grad_(True)
-    outs = _outputs(m.forward_from_srt(t["pts"], t["means"], t["opa"], t["sem"], s_d, r_d))
-    ref = h.oracle_forward(kw, inp, variant)
-    _check_forward(outs, ref, variant, f"{variant}/srt", rtol=1e-3, atol=1e-4)   # Sigma^-1 built in fp32 on the device
-    g, dev = _upstream(outs, 29)
-    torch.autograd.backward(list(outs), dev)
-    g64, _ = h.oracle_grads(kw, inp, variant, tuple(x.numpy() for x in g), _saved(outs, kw, inp, variant))
-    s64 = inp["scales"][0].double().requires_grad_(True)
-    r64 = rots[0].double().requires_grad_(True)
-    ref_s, ref_r = torch.autograd.grad(inverse_covariance_from_srt(s64, r64), (s64, r64),
-                                       torch.from_numpy(np.asarray(g64["cov"], np.float64)))
-    for name, mine, want in (("scales", s_d.grad[0], ref_s), ("rotations", r_d.grad[0], ref_r)):
-        want = want.numpy()
-        h.assert_close(mine.cpu().numpy(), want, rtol=2e-3, atol=2e-4 * max(1.0, float(np.abs(want).max())),
-                       what=f"{variant}/srt grad {name}")
+    inp = dict(inp, pts=inp["pts"][:, perm].contiguous())
+    srt.check_srt(kw, inp, rots, variant, f"{variant}/srt", det=torch.are_deterministic_algorithms_enabled())
 
 
 # ------------------------------------------------------------------------------------------------ permutation invariance
