@@ -11,7 +11,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-SOURCES = ["cabi.cu", "splat_prep.cu", "splat_forward.cu", "splat_backward.cu", "splat_backward_bin.cu", "daf.cu", "daf_fused.cu", "daf_det.cu", "daf_project.cu", "daf_anchor.cu"]
+SOURCES = ["cabi.cu", "splat_prep.cu", "splat_forward.cu", "splat_backward.cu", "splat_backward_bin.cu", "daf.cu", "daf_fused.cu", "daf_det.cu", "daf_project.cu", "daf_anchor.cu", "occ_loss.cu"]
 LIB = os.path.join(HERE, "libgf_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
@@ -27,7 +27,7 @@ def _stale() -> bool:
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(HERE, f) for f in SOURCES + ["common.cuh", "splat_render.cuh", "splat_tile.cuh", "splat_bwd_common.cuh", "splat_host.cuh", "daf_pair.cuh"]] + [os.path.join(ROOT, "include", "gf_b200.h"), os.path.join(ROOT, "include", "gf_b200_debug.h")]
+    deps = [os.path.join(HERE, f) for f in SOURCES + ["common.cuh", "splat_render.cuh", "splat_tile.cuh", "splat_bwd_common.cuh", "splat_host.cuh", "daf_pair.cuh", "radix_sort.cuh"]] + [os.path.join(ROOT, "include", "gf_b200.h"), os.path.join(ROOT, "include", "gf_b200_debug.h")]
     return any(os.path.getmtime(d) > t for d in deps)
 
 

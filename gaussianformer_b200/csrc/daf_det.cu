@@ -19,14 +19,11 @@
 #include <algorithm>
 
 #include "daf_pair.cuh"
+#include "radix_sort.cuh"
 
 namespace gf {
 namespace {
 
-constexpr int kScanThreads = 256, kScanItems = 16, kScanTile = kScanThreads * kScanItems;
-constexpr int kSortThreads = 256, kSortWarps = kSortThreads / 32, kSortIters = 16;
-constexpr int kSortTile = kSortWarps * 32 * kSortIters;   // entries per sort tile; a warp owns 32 * kSortIters of them
-constexpr int kRadixBits = 8, kRadix = 1 << kRadixBits;
 constexpr size_t kAlign = 256;
 
 // The workspace of the route, from the desc alone.  Cells: level l of (b, m) starts at sum_{k<l} (h_k+1)(w_k+1) of
@@ -93,80 +90,6 @@ struct DetParams {
     int *hist;                  // [kRadix, tiles]: digit-major, so one exclusive scan gives every (digit, tile) its start
     int *cell_start, *cell_end; // [ncells]: entry range of a cell in the sorted order (0, 0 = empty)
 };
-
-// ---------------------------------------------------------------------------------------------------------- scans
-// Exclusive scan of kScanThreads values of one block; `total` receives their sum.
-__device__ __forceinline__ int block_exclusive_scan(int v, int &total) {
-    __shared__ int s_warp[kScanThreads / 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += t;
-    }
-    if (lane == 31) s_warp[warp] = inc;
-    __syncthreads();
-    int off = 0;
-    total = 0;
-#pragma unroll
-    for (int w = 0; w < kScanThreads / 32; ++w) {
-        const int c = s_warp[w];
-        if (w < warp) off += c;
-        total += c;
-    }
-    __syncthreads();
-    return off + inc - v;
-}
-
-__global__ void __launch_bounds__(kScanThreads) scan_reduce_kernel(const int *data, long long n, int *partials) {
-    const long long base = static_cast<long long>(blockIdx.x) * kScanTile;
-    int s = 0;
-    for (int i = threadIdx.x; i < kScanTile; i += kScanThreads)
-        if (base + i < n) s += data[base + i];
-    int total;
-    block_exclusive_scan(s, total);
-    if (threadIdx.x == 0) partials[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(kScanThreads) scan_partials_kernel(int *partials, int n) {
-    int carry = 0;
-    for (int base = 0; base < n; base += kScanThreads) {
-        const int i = base + threadIdx.x;
-        const int v = i < n ? partials[i] : 0;
-        int total;
-        const int ex = block_exclusive_scan(v, total);
-        if (i < n) partials[i] = carry + ex;
-        carry += total;
-    }
-}
-
-__global__ void __launch_bounds__(kScanThreads) scan_apply_kernel(int *data, long long n, const int *partials) {
-    const long long base = static_cast<long long>(blockIdx.x) * kScanTile + threadIdx.x * kScanItems;
-    int v[kScanItems], s = 0;
-#pragma unroll
-    for (int k = 0; k < kScanItems; ++k) {
-        v[k] = base + k < n ? data[base + k] : 0;
-        s += v[k];
-    }
-    int total;
-    int run = partials[blockIdx.x] + block_exclusive_scan(s, total);
-#pragma unroll
-    for (int k = 0; k < kScanItems; ++k) {
-        if (base + k < n) data[base + k] = run;
-        run += v[k];
-    }
-}
-
-// in place, over n ints (an integer scan: its result does not depend on the launch)
-int exclusive_scan(int *data, long long n, int *partials, cudaStream_t stream) {
-    const long long blocks = (n + kScanTile - 1) / kScanTile;
-    scan_reduce_kernel<<<static_cast<unsigned>(blocks), kScanThreads, 0, stream>>>(data, n, partials);
-    scan_partials_kernel<<<1, kScanThreads, 0, stream>>>(partials, static_cast<int>(blocks));
-    scan_apply_kernel<<<static_cast<unsigned>(blocks), kScanThreads, 0, stream>>>(data, n, partials);
-    GF_CUDA_TRY(cudaGetLastError());
-    return GF_OK;
-}
 
 // ---------------------------------------------------------------------------------------------------------- compact
 // Level table plus the first cell of every level inside a (b, m) block (le); every thread of the block must call it.
@@ -235,66 +158,15 @@ __global__ void __launch_bounds__(kDafThreads) det_emit_kernel(const DetParams p
 
 // ---------------------------------------------------------------------------------------------------------- sort
 __global__ void __launch_bounds__(kSortThreads) radix_hist_kernel(const DetParams p, const uint32_t *keys, int shift) {
-    __shared__ int cnt[kRadix];
-    for (int i = threadIdx.x; i < kRadix; i += kSortThreads) cnt[i] = 0;
-    __syncthreads();
-    const long long n = p.counts[static_cast<long long>(p.d.batch) * p.d.num_pts];
-    const long long t0 = static_cast<long long>(blockIdx.x) * kSortTile;
-    for (int i = threadIdx.x; i < kSortTile; i += kSortThreads)
-        if (t0 + i < n) atomicAdd(&cnt[(keys[t0 + i] >> shift) & (kRadix - 1)], 1);
-    __syncthreads();
-    for (int dg = threadIdx.x; dg < kRadix; dg += kSortThreads) p.hist[static_cast<long long>(dg) * p.tiles + blockIdx.x] = cnt[dg];
+    const auto count = [&] { return static_cast<long long>(p.counts[static_cast<long long>(p.d.batch) * p.d.num_pts]); };
+    radix_tile_hist(keys, count, shift, p.hist, p.tiles, blockIdx.x);
 }
 
-// Stable scatter of one tile: warp w owns the tile's w-th run of 32 * kSortIters entries.  Pass 1 counts each warp's
-// digits, then every digit's start is the tile's scanned offset plus the counts of the warps before; pass 2 places
-// each entry after the equal digits of its warp's earlier entries and of the lanes below it (__match_any_sync).
 __global__ void __launch_bounds__(kSortThreads) radix_scatter_kernel(const DetParams p, const uint32_t *keys_in,
                                                                      const int *vals_in, uint32_t *keys_out,
                                                                      int *vals_out, int shift) {
-    __shared__ int wcnt[kSortWarps][kRadix];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const long long n = p.counts[static_cast<long long>(p.d.batch) * p.d.num_pts];
-    const long long t0 = static_cast<long long>(blockIdx.x) * kSortTile;
-    if (t0 >= n) return;   // uniform over the block
-    const long long w0 = t0 + static_cast<long long>(warp) * 32 * kSortIters;
-    for (int i = lane; i < kRadix; i += 32) wcnt[warp][i] = 0;
-    __syncwarp();
-    for (int it = 0; it < kSortIters; ++it) {
-        const long long j = w0 + it * 32 + lane;
-        const int dg = j < n ? static_cast<int>((keys_in[j] >> shift) & (kRadix - 1)) : kRadix;
-        const uint32_t peers = __match_any_sync(0xffffffffu, dg);
-        if (dg < kRadix && lane == __ffs(peers) - 1) wcnt[warp][dg] += __popc(peers);
-        __syncwarp();
-    }
-    __syncthreads();
-    for (int dg = threadIdx.x; dg < kRadix; dg += kSortThreads) {
-        int run = p.hist[static_cast<long long>(dg) * p.tiles + blockIdx.x];
-        for (int w = 0; w < kSortWarps; ++w) {
-            const int c = wcnt[w][dg];
-            wcnt[w][dg] = run;
-            run += c;
-        }
-    }
-    __syncthreads();
-    for (int it = 0; it < kSortIters; ++it) {
-        const long long j = w0 + it * 32 + lane;
-        uint32_t key = 0;
-        int dg = kRadix;
-        if (j < n) {
-            key = keys_in[j];
-            dg = static_cast<int>((key >> shift) & (kRadix - 1));
-        }
-        const uint32_t peers = __match_any_sync(0xffffffffu, dg);
-        if (dg < kRadix) {
-            const int at = wcnt[warp][dg] + __popc(peers & lanemask_lt());
-            keys_out[at] = key;
-            vals_out[at] = vals_in[j];
-        }
-        __syncwarp();
-        if (dg < kRadix && lane == __ffs(peers) - 1) wcnt[warp][dg] += __popc(peers);
-        __syncwarp();
-    }
+    const auto count = [&] { return static_cast<long long>(p.counts[static_cast<long long>(p.d.batch) * p.d.num_pts]); };
+    radix_tile_scatter(keys_in, vals_in, keys_out, vals_out, count, shift, p.hist, p.tiles, blockIdx.x);
 }
 
 __global__ void __launch_bounds__(256) cell_bounds_kernel(const DetParams p, const uint32_t *keys) {

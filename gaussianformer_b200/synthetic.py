@@ -386,3 +386,46 @@ def reference_fused_composition(daf_apply, feat, shape, start, loc, logits, poin
     weights = weights * (1 - all_miss.flatten(1, 2).float())
     features = daf_apply(feat, shape, start, loc, weights).reshape(B, A, K, -1)
     return features.sum(dim=2)
+
+
+# Label shares of a SurroundOcc-like occupancy target: class 17 (empty) dominates, a few percent are class 0 (others),
+# the rest spread unevenly over the semantic classes 1..16.  These shares are an assumption -- real label statistics
+# are not part of this repository -- chosen so that every class is present at full size and the Lovasz sort sees the
+# heavy class imbalance of an occupancy grid.
+OCC_EMPTY_SHARE, OCC_ZERO_SHARE = 0.88, 0.03
+
+
+def make_occ_labels(batch, n, num_classes=18, seed=0, ignore_share=0.0, generator=None):
+    """``[batch, n]`` int64 labels: ``OCC_EMPTY_SHARE`` of ``num_classes - 1``, ``OCC_ZERO_SHARE`` of 0, the rest over
+    1..num_classes-2 with weights 1..num_classes-2 (uneven on purpose), and ``ignore_share`` of 255."""
+    g = generator or torch.Generator().manual_seed(seed)
+    sem = num_classes - 2
+    probs = torch.tensor([OCC_ZERO_SHARE] + [(1 - OCC_EMPTY_SHARE - OCC_ZERO_SHARE) * (k + 1) / (sem * (sem + 1) / 2)
+                                             for k in range(sem)] + [OCC_EMPTY_SHARE], dtype=torch.float64)
+    labels = torch.multinomial(probs, batch * n, replacement=True, generator=g).reshape(batch, n)
+    if ignore_share > 0:
+        labels[torch.rand(batch, n, generator=g) < ignore_share] = 255
+    return labels
+
+
+def make_occ_loss_inputs(batch=1, n=640000, num_classes=18, use_softmax=True, seed=0, ignore_share=0.0,
+                         duplicate_share=0.01, mask=True):
+    """Inputs of ``occupancy_loss`` as the head hands them over: ``pred`` ``[B, N, C]`` fp32 contiguous (the splat's
+    output; the loss takes ``pred.transpose(1, 2)``), logits ~ 2 N(0, 1) with the label's class raised by 1, or their
+    fp32 softmax for the probability branch; ``labels`` ``[B, N]`` int64 (make_occ_labels); ``occ_mask`` ``[B, N]`` bool
+    = ``labels != 0`` as the loader builds it, or None.  ``duplicate_share`` of the voxels copy the prediction and the
+    label of an earlier voxel bit for bit, so the Lovasz sort meets exact ties at every size."""
+    g = torch.Generator().manual_seed(seed)
+    labels = make_occ_labels(batch, n, num_classes, generator=g, ignore_share=ignore_share)
+    logits = 2.0 * torch.randn(batch, n, num_classes, generator=g)
+    lab = labels.clamp(max=num_classes - 1)
+    logits.scatter_add_(2, lab[..., None], torch.ones(batch, n, 1))
+    pred = torch.softmax(logits, dim=2) if not use_softmax else logits
+    ndup = int(duplicate_share * n)
+    if ndup > 0 and n > 1:
+        dst = torch.randperm(n, generator=g)[:ndup]
+        src = (torch.rand(ndup, generator=g) * dst.float()).long()   # an earlier voxel (dst 0 copies itself)
+        pred[:, dst] = pred[:, src]
+        labels[:, dst] = labels[:, src]
+    occ_mask = labels != 0 if mask else None
+    return pred.contiguous(), labels, occ_mask

@@ -408,6 +408,59 @@ int gf_daf_anchor_key_points_backward(const gf_daf_kps_desc *desc, const float *
                                       const float *learnable_logits, const float *grad_key_points,
                                       float *grad_anchor, float *grad_learnable, gf_stream_t stream);
 
+/* ---- occupancy loss of one supervised layer: OccupancyLoss.loss_voxel (loss/occupancy_loss.py:102-149) as every
+ * shipped config runs it, ce_weight * CE + lovasz_weight * Lovasz-softmax (loss/utils/lovasz_softmax.py:157-234),
+ * with its gradient.  Inputs: pred [B, C, N] (logits, or probabilities with GF_OCC_PROBS) in one of two layouts,
+ * labels [B, N] int64, mask [B, N] bytes or NULL (all voxels), class_weights [C].
+ *
+ *   S   = {(b, n) : mask, and label != empty_label when empty_label >= 0}, b-major, n ascending (one pool: B > 1 is
+ *         the batch pooled, not averaged per sample)
+ *   CE  = sum w[y] (-log p_y) / sum w[y] over the s in S with y != ignore_index; p = softmax_c(pred) (GF_OCC_LOGITS)
+ *         or clamp(pred, 1e-6f, 1 - 1e-6f) (GF_OCC_PROBS).  NaN when no voxel counts, as PyTorch's mean
+ *   V   = {s in S : y != lovasz_ignore} in S order; r = p (GF_OCC_LOGITS) or pred (GF_OCC_PROBS).  A label outside
+ *         [0, C) stays in V as background of every class.  Class c is present if some s in V has y = c.  For each:
+ *         e_s = |[y_s = c] - r_{s,c}| sorted descending, equal errors in ascending position in V (a stable sort);
+ *         fg in that order, G = sum fg, I_k = G - sum_{j<=k} fg_j, U_k = G + sum_{j<=k} (1 - fg_j),
+ *         J_k = 1 - I_k / U_k, Delta_k = J_k - J_{k-1} (J_{-1} = 0), L_c = sum_k e_(k) Delta_k.
+ *         Lovasz = mean of L_c over the present classes, 0 when none is
+ *   loss_out[3] = { weight * (ce_weight * CE + lovasz_weight * Lovasz), CE, Lovasz }, fully overwritten
+ *
+ * grad_out (NULL: loss only) receives d loss_out[0] / d pred in pred's layout, every entry written (0 outside S).  No
+ * gradient flows through Delta, and |.| at 0 passes 0 (torch.abs).  The arithmetic is fp64 from the fp32 inputs; each
+ * error is rounded to fp32 once to be sorted, and the loss and every gradient entry once at the end.  Every sum runs
+ * in a fixed order without floating-point atomics, so loss and gradient are bit-reproducible from call to call.
+ *
+ * The workspace is sized from the desc for the worst case |V| = B * N (gf_occ_loss_workspace_bytes; 16 * C * B * N
+ * bytes for the sort plus O(B * N) more), 256-byte aligned; the counts stay on the device, so the call never
+ * synchronises and can be captured in a CUDA graph.  The first uint32 of the workspace is the call's status word:
+ * GF_FLAG_LABEL_OUT_OF_RANGE when a label in S is outside [0, C) and neither ignore_index nor lovasz_ignore.
+ *
+ * Supported: C in gf_splat_supported_classes(), B * N * C < 2^31.  Otherwise, and for a NULL desc, unknown branch or
+ * layout, NULL pointers or a small workspace, the call fails before any CUDA call. */
+#define GF_OCC_LOGITS 0
+#define GF_OCC_PROBS 1
+#define GF_OCC_VOXEL_MAJOR 0   /* pred[b, c, n] at (b * N + n) * C + c: the transposed view of the splat's [B, N, C] */
+#define GF_OCC_CLASS_MAJOR 1   /* pred[b, c, n] at (b * C + c) * N + n: the contiguous [B, C, N] of logits_cn */
+#define GF_FLAG_LABEL_OUT_OF_RANGE 8u
+
+typedef struct gf_occ_loss_desc {
+    int32_t batch;         /* B */
+    int32_t N;             /* voxels per sample */
+    int32_t C;             /* classes */
+    int32_t branch;        /* GF_OCC_LOGITS | GF_OCC_PROBS */
+    int32_t layout;        /* GF_OCC_VOXEL_MAJOR | GF_OCC_CLASS_MAJOR, for pred and grad_out */
+    int32_t ignore_index;  /* CE ignore label (255) */
+    int32_t lovasz_ignore; /* label left out of V (17 in the shipped configs) */
+    int32_t empty_label;   /* ignore_empty: voxels with this label leave S; < 0 = off */
+    float weight, ce_weight, lovasz_weight;
+} gf_occ_loss_desc;
+
+size_t gf_occ_loss_workspace_bytes(const gf_occ_loss_desc *desc);
+
+int gf_occ_loss(const gf_occ_loss_desc *desc, const float *pred, const int64_t *labels, const uint8_t *mask,
+                const float *class_weights, float *loss_out, float *grad_out, void *workspace, size_t workspace_bytes,
+                gf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -43,6 +43,13 @@ int gf_debug_splat_backward_route(const gf_splat_desc *desc, const void *workspa
  * backwards, both routes); <= 0: back to the device's.  For tests of results that must not depend on the GPU size. */
 int gf_debug_daf_plan(int32_t num_sms);
 
+/* The sorted order of the last gf_occ_loss that used `workspace` (same desc): *host_num_v = |V|, host_present[c]
+ * (C bytes) whether class c was present, and for each present class row c of host_order [C, B * N] receives, in its
+ * first |V| entries, the positions in V of the errors in sorted order (other entries are left as they are).
+ * Synchronises the stream. */
+int gf_debug_occ_loss_order(const gf_occ_loss_desc *desc, const void *workspace, gf_stream_t stream,
+                            int32_t *host_order, int32_t *host_num_v, uint8_t *host_present);
+
 #ifdef __cplusplus
 }
 #endif
