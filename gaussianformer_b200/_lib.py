@@ -20,18 +20,22 @@ GF_FLAG_MEAN_OUT_OF_GRID = 2
 GF_FLAG_RADIUS_LT_1 = 4
 GF_FLAG_GENERIC_PATH = 256
 GF_ERR_INVALID_ARG = 1
+GF_ERR_WORKSPACE = 2
 GF_ERR_UNSUPPORTED = 4
 GF_DTYPE_F32, GF_DTYPE_F16, GF_DTYPE_BF16 = 0, 1, 2
 GF_BWD_DETERMINISTIC = 1
 GF_OCC_LOGITS, GF_OCC_PROBS = 0, 1
 GF_OCC_VOXEL_MAJOR, GF_OCC_CLASS_MAJOR = 0, 1
 GF_FLAG_LABEL_OUT_OF_RANGE = 8
+GF_FLAG_INDEX_OUT_OF_RANGE = 16
+GF_SUBM_DW_PIECES = 8
 # include/gf_b200_debug.h: route word of a deterministic backward
 GF_DEBUG_ROUTE_BIN, GF_DEBUG_ROUTE_SLOT_OVERFLOW, GF_DEBUG_ROUTE_STRAY_POINTS, GF_DEBUG_ROUTE_GAUSSIAN = 0, 1, 2, 3
 
 # include/gf_b200_debug.h: measurement hooks, not the drop-in boundary
 DEBUG_EXPORTS = ("gf_debug_set_render_events", "gf_debug_gather_probe", "gf_debug_splat_backward_plan",
-                 "gf_debug_splat_backward_route", "gf_debug_daf_plan", "gf_debug_occ_loss_order")
+                 "gf_debug_splat_backward_route", "gf_debug_daf_plan", "gf_debug_occ_loss_order",
+                 "gf_debug_subm_conv_neighbors")
 EXPORTS = (
     "gf_abi_version", "gf_last_error", "gf_splat_supported_classes",
     "gf_splat_forward_workspace_bytes", "gf_splat_backward_workspace_bytes",
@@ -44,6 +48,7 @@ EXPORTS = (
     "gf_daf_fused_backward_ex2", "gf_daf_project", "gf_daf_project_backward",
     "gf_daf_anchor_key_points", "gf_daf_anchor_key_points_backward",
     "gf_occ_loss_workspace_bytes", "gf_occ_loss",
+    "gf_subm_conv_workspace_bytes", "gf_subm_conv_rulebook", "gf_subm_conv_forward", "gf_subm_conv_backward",
 )
 
 
@@ -100,6 +105,11 @@ class OccLossDesc(Structure):
     _fields_ = [("batch", c_int32), ("N", c_int32), ("C", c_int32), ("branch", c_int32), ("layout", c_int32),
                 ("ignore_index", c_int32), ("lovasz_ignore", c_int32), ("empty_label", c_int32),
                 ("weight", c_float), ("ce_weight", c_float), ("lovasz_weight", c_float)]
+
+
+class SubmConvDesc(Structure):
+    _fields_ = [("batch", c_int32), ("num_rows", c_int32), ("X", c_int32), ("Y", c_int32), ("Z", c_int32),
+                ("kernel_size", c_int32), ("c_in", c_int32), ("c_out", c_int32)]
 
 
 class GfError(RuntimeError):
@@ -167,6 +177,12 @@ def lib():
         L.gf_occ_loss_workspace_bytes.argtypes = [POINTER(OccLossDesc)]
         L.gf_occ_loss.argtypes = [POINTER(OccLossDesc)] + [c_void_p] * 7 + [c_size_t, c_void_p]
         L.gf_debug_occ_loss_order.argtypes = [POINTER(OccLossDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
+        L.gf_subm_conv_workspace_bytes.restype = c_size_t
+        L.gf_subm_conv_workspace_bytes.argtypes = [POINTER(SubmConvDesc)]
+        L.gf_subm_conv_rulebook.argtypes = [POINTER(SubmConvDesc), c_void_p, c_void_p, c_size_t, c_void_p]
+        L.gf_subm_conv_forward.argtypes = [POINTER(SubmConvDesc)] + [c_void_p] * 6
+        L.gf_subm_conv_backward.argtypes = [POINTER(SubmConvDesc)] + [c_void_p] * 8
+        L.gf_debug_subm_conv_neighbors.argtypes = [POINTER(SubmConvDesc)] + [c_void_p] * 6
         if L.gf_abi_version() != 2:
             raise ImportError("libgf_b200.so: ABI version mismatch")
         _lib = L

@@ -429,3 +429,61 @@ def make_occ_loss_inputs(batch=1, n=640000, num_classes=18, use_softmax=True, se
         labels[:, dst] = labels[:, src]
     occ_mask = labels != 0 if mask else None
     return pred.contiguous(), labels, occ_mask
+
+
+# Assumed shares of the clustered sparse-convolution anchors: trained Gaussians gather on surfaces, here a ground
+# plane (SUBM_GROUND_SHARE, in the lowest SUBM_GROUND_LEVELS z levels) and the faces of SUBM_BOXES boxes (the rest).
+# These are assumptions standing in for a trained model's anchors, not measured statistics.
+SUBM_GROUND_SHARE, SUBM_GROUND_LEVELS, SUBM_BOXES = 0.5, 2, 24
+
+
+def make_subm_conv_inputs(n, spatial, batch=1, clustered=False, seed=0, kernel_size=5, channels=128,
+                          invalid=0, duplicates_of=None):
+    """Inputs of ``subm_conv3d``: ``features [N, C]`` ~ N(0, 1), ``indices [N, 4]`` int32 rows ``(b, x, y, z)``
+    (``n`` rows per sample, b-major, then shuffled), ``weight [C, k, k, k, C]`` and ``bias [C]`` ~ U(+-1/sqrt(k^3 C))
+    as nn.Conv3d initialises them.  Voxels are uniform over the grid, or with ``clustered`` on the ground plane and box
+    faces (shares above).  ``invalid`` rows get an out-of-grid coordinate or batch index; ``duplicates_of`` = m puts
+    every m-th row into the voxel of one of the first N / 4m rows, about four per voxel, so that some voxels hold 3
+    or more rows."""
+    g = torch.Generator().manual_seed(seed)
+    X, Y, Z = spatial
+    rows = []
+    for b in range(batch):
+        nb = n if isinstance(n, int) else n[b]
+        if clustered:
+            ng = int(SUBM_GROUND_SHARE * nb)
+            ground = torch.stack([torch.randint(0, X, (ng,), generator=g), torch.randint(0, Y, (ng,), generator=g),
+                                  torch.randint(0, SUBM_GROUND_LEVELS, (ng,), generator=g)], 1)
+            lo = torch.stack([torch.randint(0, X, (SUBM_BOXES,), generator=g), torch.randint(0, Y, (SUBM_BOXES,), generator=g),
+                              torch.randint(0, max(1, Z // 2), (SUBM_BOXES,), generator=g)], 1)
+            size = torch.stack([torch.randint(4, max(5, X // 8), (SUBM_BOXES,), generator=g),
+                                torch.randint(4, max(5, Y // 8), (SUBM_BOXES,), generator=g),
+                                torch.randint(2, max(3, Z // 2), (SUBM_BOXES,), generator=g)], 1)
+            nf = nb - ng
+            box = torch.randint(0, SUBM_BOXES, (nf,), generator=g)
+            u = torch.rand(nf, 3, generator=g)
+            face = torch.randint(0, 6, (nf,), generator=g)
+            u[torch.arange(nf), face // 2] = (face % 2).float()            # pin one coordinate to a face
+            pts = lo[box] + (u * (size[box] - 1).float()).round().long()
+            pts = torch.minimum(pts, torch.tensor([X - 1, Y - 1, Z - 1]))
+            xyz = torch.cat([ground, pts], 0)
+        else:
+            xyz = torch.stack([torch.randint(0, X, (nb,), generator=g), torch.randint(0, Y, (nb,), generator=g),
+                               torch.randint(0, Z, (nb,), generator=g)], 1)
+        rows.append(torch.cat([torch.full((xyz.shape[0], 1), b, dtype=torch.long), xyz], 1))
+    idx = torch.cat(rows, 0)
+    N = idx.shape[0]
+    if duplicates_of:
+        dst = torch.arange(duplicates_of, N, duplicates_of)
+        idx[dst] = idx[(dst // duplicates_of) % max(1, N // (4 * duplicates_of))]   # ~4 copies of each early row
+    if invalid:
+        bad = torch.randperm(N, generator=g)[:invalid]
+        col = torch.randint(0, 4, (invalid,), generator=g)
+        lim = torch.tensor([batch, X, Y, Z])
+        idx[bad, col] = torch.where(torch.rand(invalid, generator=g) < 0.5, -1 - col, lim[col] + col)
+    idx = idx[torch.randperm(N, generator=g)].to(torch.int32).contiguous()
+    bound = 1.0 / math.sqrt(kernel_size ** 3 * channels)
+    features = torch.randn(N, channels, generator=g)
+    weight = (torch.rand(channels, kernel_size, kernel_size, kernel_size, channels, generator=g) * 2 - 1) * bound
+    bias = (torch.rand(channels, generator=g) * 2 - 1) * bound
+    return features, idx, weight, bias

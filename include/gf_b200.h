@@ -461,6 +461,65 @@ int gf_occ_loss(const gf_occ_loss_desc *desc, const float *pred, const int64_t *
                 const float *class_weights, float *loss_out, float *grad_out, void *workspace, size_t workspace_bytes,
                 gf_stream_t stream);
 
+/* ---- submanifold sparse convolution: spconv's SubMConv3d(c_in, c_out, k, stride 1, padding (k-1)/2) as the
+ * encoder's SparseConv3D (model/encoder/gaussian_encoder/spconv3d_module.py:10-83) calls it, forward and backward.
+ * Inputs: features [N, c_in] fp32, indices [N, 4] int32 rows (b, x, y, z) in any order, weight in spconv 2.x layout
+ * [c_out, k, k, k, c_in], bias [c_out] or NULL.
+ *
+ *   valid row   0 <= b < batch and (x, y, z) inside [0, X) x [0, Y) x [0, Z)
+ *   voxel       occupied when it holds a valid row; rep(v) = the LOWEST valid row index in it.  spconv keeps one row
+ *               per voxel too but leaves open which; fixing the lowest is this op's documented deviation
+ *   offset      o = (a * k + c) * k + e, a, c, e in [0, k), delta_o = (a - p, c - p, e - p) over (x, y, z), p = (k-1)/2
+ *   out[i]      = bias + sum_o W[:, a, c, e, :] . features[rep(v + delta_o)] for every valid row i in voxel v, summed
+ *               over the o whose target voxel is occupied (a cross-correlation, as nn.Conv3d).  Every row of a voxel
+ *               gets the same output bit for bit.  Invalid rows get 0 (no bias) and contribute nothing.
+ *
+ * Backward: exact gradients of the above.  grad_features is the gradient at representative rows and exactly 0 at
+ * every other row; grad_weight has weight's layout; grad_bias = sum over valid rows of grad_out.  Any of the three may
+ * be NULL (not computed).  fp32 throughout (no TF32), no floating-point atomics: every sum runs in a fixed order
+ * (offsets ascending; the rows of a voxel ascending; grad_weight in GF_SUBM_DW_PIECES fixed split-K pieces per offset,
+ * summed in piece order), so the output and the three gradients are bit-reproducible from call to call.
+ *
+ * gf_subm_conv_rulebook builds, from indices alone, the voxel table, the representatives, the [k^3, N] neighbour table,
+ * the per-offset pair lists and the rows grouped by voxel; one rulebook serves any number of forward and backward
+ * calls on the same indices and desc.  The forward and backward calls also use the workspace for their own scratch,
+ * so calls that share a workspace must be ordered (one stream).  Counts stay on the device and the workspace is sized
+ * from the desc for the worst case (every row its own voxel), so nothing synchronises and the calls can be captured
+ * in a CUDA graph.  With V = batch * X * Y * Z, K = k^3, C = 128 (c_in = c_out), P = GF_SUBM_DW_PIECES, the workspace
+ * is, up to 256-byte alignment and a few small arrays,
+ *
+ *   8 V + 4 N (8 + 2 K + 2 C) + 4 K C^2 (1 + P) bytes
+ *
+ * (375 MB for N = 144 000 rows on one 200 x 200 x 16 sample with k = 5).  The first uint32 of the workspace is the
+ * status word: the rulebook sets GF_FLAG_INDEX_OUT_OF_RANGE when a row is invalid.
+ *
+ * Supported: c_in = c_out = 128 (GF_ERR_UNSUPPORTED otherwise), odd k <= 5, batch, X, Y, Z, N >= 1; V, N * K and
+ * N * C each < 2^31 (GF_ERR_UNSUPPORTED otherwise).  A NULL desc or pointer, an even or larger k, non-positive sizes,
+ * indices, features, out, grad_out or grad_features not 16-byte aligned, or a workspace that is NULL, misaligned or
+ * smaller than the query fail before any CUDA call. */
+#define GF_FLAG_INDEX_OUT_OF_RANGE 16u
+#define GF_SUBM_DW_PIECES 8
+
+typedef struct gf_subm_conv_desc {
+    int32_t batch;         /* B */
+    int32_t num_rows;      /* N */
+    int32_t X, Y, Z;       /* spatial shape, over index columns 1, 2, 3 */
+    int32_t kernel_size;   /* k: 1, 3 or 5 */
+    int32_t c_in, c_out;   /* 128 */
+} gf_subm_conv_desc;
+
+size_t gf_subm_conv_workspace_bytes(const gf_subm_conv_desc *desc);
+
+int gf_subm_conv_rulebook(const gf_subm_conv_desc *desc, const int32_t *indices, void *workspace,
+                          size_t workspace_bytes, gf_stream_t stream);
+
+int gf_subm_conv_forward(const gf_subm_conv_desc *desc, void *workspace, const float *features, const float *weight,
+                         const float *bias, float *out, gf_stream_t stream);
+
+int gf_subm_conv_backward(const gf_subm_conv_desc *desc, void *workspace, const float *features, const float *weight,
+                          const float *grad_out, float *grad_features, float *grad_weight, float *grad_bias,
+                          gf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -50,6 +50,14 @@ int gf_debug_daf_plan(int32_t num_sms);
 int gf_debug_occ_loss_order(const gf_occ_loss_desc *desc, const void *workspace, gf_stream_t stream,
                             int32_t *host_order, int32_t *host_num_v, uint8_t *host_present);
 
+/* The rulebook gf_subm_conv_rulebook left in `workspace` (same desc): *host_num_voxels = M, the occupied voxels;
+ * host_slot[N] the voxel slot of every row (slots number the occupied voxels in ascending (b, x, y, z) order; -1 for an
+ * invalid row); host_rep[N] the representative row of every slot in its first M entries; host_nbr [N, k^3] in its
+ * first M rows the slot of the neighbour at every offset, or -1.  Entries past M are left as they are.  Synchronises
+ * the stream. */
+int gf_debug_subm_conv_neighbors(const gf_subm_conv_desc *desc, const void *workspace, gf_stream_t stream,
+                                 int32_t *host_num_voxels, int32_t *host_slot, int32_t *host_rep, int32_t *host_nbr);
+
 #ifdef __cplusplus
 }
 #endif
