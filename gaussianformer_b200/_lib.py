@@ -29,6 +29,9 @@ GF_OCC_VOXEL_MAJOR, GF_OCC_CLASS_MAJOR = 0, 1
 GF_FLAG_LABEL_OUT_OF_RANGE = 8
 GF_FLAG_INDEX_OUT_OF_RANGE = 16
 GF_SUBM_DW_PIECES = 8
+GF_REFINE_V1, GF_REFINE_V2 = 0, 1
+GF_REFINE_IDENTITY, GF_REFINE_SOFTMAX, GF_REFINE_SOFTPLUS = 0, 1, 2
+GF_REFINE_MAX_SEMANTICS = 32
 # include/gf_b200_debug.h: route word of a deterministic backward
 GF_DEBUG_ROUTE_BIN, GF_DEBUG_ROUTE_SLOT_OVERFLOW, GF_DEBUG_ROUTE_STRAY_POINTS, GF_DEBUG_ROUTE_GAUSSIAN = 0, 1, 2, 3
 
@@ -49,6 +52,7 @@ EXPORTS = (
     "gf_daf_anchor_key_points", "gf_daf_anchor_key_points_backward",
     "gf_occ_loss_workspace_bytes", "gf_occ_loss",
     "gf_subm_conv_workspace_bytes", "gf_subm_conv_rulebook", "gf_subm_conv_forward", "gf_subm_conv_backward",
+    "gf_gaussian_refine", "gf_gaussian_refine_backward",
 )
 
 
@@ -110,6 +114,26 @@ class OccLossDesc(Structure):
 class SubmConvDesc(Structure):
     _fields_ = [("batch", c_int32), ("num_rows", c_int32), ("X", c_int32), ("Y", c_int32), ("Z", c_int32),
                 ("kernel_size", c_int32), ("c_in", c_int32), ("c_out", c_int32)]
+
+
+class RefineDesc(Structure):
+    _fields_ = [("variant", c_int32), ("batch", c_int32), ("num_anchors", c_int32), ("out_dim", c_int32),
+                ("anchor_dim", c_int32), ("refine_prefix", c_int32), ("restrict_xyz", c_int32),
+                ("include_opa", c_int32), ("semantic_dim", c_int32), ("semantics_act", c_int32),
+                ("lo", c_float * 3), ("extent", c_float * 3), ("unit", c_float * 3), ("scale_lo", c_float),
+                ("scale_extent", c_float)]
+
+
+REFINE_OUTPUTS = ("new_anchor", "means", "scales", "rotations", "opacities", "semantics", "original_means",
+                  "delta_means")
+
+
+class RefineOutputs(Structure):
+    _fields_ = [(n, c_void_p) for n in REFINE_OUTPUTS]
+
+
+class RefineGrads(Structure):
+    _fields_ = [(n, c_void_p) for n in REFINE_OUTPUTS]
 
 
 class GfError(RuntimeError):
@@ -183,6 +207,9 @@ def lib():
         L.gf_subm_conv_forward.argtypes = [POINTER(SubmConvDesc)] + [c_void_p] * 6
         L.gf_subm_conv_backward.argtypes = [POINTER(SubmConvDesc)] + [c_void_p] * 8
         L.gf_debug_subm_conv_neighbors.argtypes = [POINTER(SubmConvDesc)] + [c_void_p] * 6
+        L.gf_gaussian_refine.argtypes = [POINTER(RefineDesc), c_void_p, c_void_p, POINTER(RefineOutputs), c_void_p]
+        L.gf_gaussian_refine_backward.argtypes = [POINTER(RefineDesc), c_void_p, c_void_p, POINTER(RefineGrads),
+                                                  c_void_p, c_void_p, c_void_p]
         if L.gf_abi_version() != 2:
             raise ImportError("libgf_b200.so: ABI version mismatch")
         _lib = L

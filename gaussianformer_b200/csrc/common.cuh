@@ -396,6 +396,22 @@ __device__ __forceinline__ void quat_rotation_backward(const T q[4], T inv_norm,
     dq[3] = inv_norm * (gz - z * dot);
 }
 
+// safe_sigmoid (model/utils/safe_ops.py:7-9) in fp64, for the key-point generator (daf_anchor.cu) and the refinement
+// (gaussian_refine.cu).  The constants are the values the reference's fp32 tensors hold.
+constexpr double kLogitClamp = static_cast<double>(9.21f);   // safe_sigmoid's bound
+constexpr double kNormEps = static_cast<double>(1e-12f);     // F.normalize's epsilon
+
+struct Sigmoid {
+    double s;    // sigmoid of the clamped logit
+    double ds;   // its derivative w.r.t. the logit: s (1 - s) inside the clamp, bounds included; 0 outside (and NaN)
+};
+
+__device__ __forceinline__ Sigmoid safe_sigmoid(double x) {
+    const double c = x < -kLogitClamp ? -kLogitClamp : (x > kLogitClamp ? kLogitClamp : x);   // NaN stays NaN
+    const double s = 1.0 / (1.0 + exp(-c));
+    return {s, (x >= -kLogitClamp && x <= kLogitClamp) ? s * (1.0 - s) : 0.0};
+}
+
 // Sigma^-1 = R^T diag(1/s^2) R as (xx,yy,zz,xy,yz,xz): the closed form of GaussianHead.prepare_gaussian_args'
 // Cov = (S R)^T (S R); Cov.cpu().inverse() (model/head/gaussian_head.py:111-119), R orthogonal.
 __device__ __forceinline__ void cov6_from_srt(const float s[3], const float q[4], float c6[6]) {

@@ -12,20 +12,6 @@
 namespace gf {
 
 constexpr int kAnchorThreads = 64;            // 25 600 anchors -> 400 CTAs: every SM gets work
-constexpr double kLogitClamp = static_cast<double>(9.21f);   // safe_sigmoid's bound as an fp32 tensor holds it
-constexpr double kNormEps = static_cast<double>(1e-12f);     // F.normalize's epsilon, likewise
-
-struct Sigmoid {
-    double s;    // sigmoid of the clamped logit
-    double ds;   // its derivative w.r.t. the logit: s (1 - s) inside the clamp, bounds included; 0 outside (and NaN)
-};
-
-__device__ __forceinline__ Sigmoid safe_sigmoid(float v) {
-    const double x = v;
-    const double c = x < -kLogitClamp ? -kLogitClamp : (x > kLogitClamp ? kLogitClamp : x);   // NaN stays NaN
-    const double s = 1.0 / (1.0 + exp(-c));
-    return {s, (x >= -kLogitClamp && x <= kLogitClamp) ? s * (1.0 - s) : 0.0};
-}
 
 struct KpsArgs {
     gf_daf_kps_desc d;

@@ -487,3 +487,113 @@ def make_subm_conv_inputs(n, spatial, batch=1, clustered=False, seed=0, kernel_s
     weight = (torch.rand(channels, kernel_size, kernel_size, kernel_size, channels, generator=g) * 2 - 1) * bound
     bias = (torch.rand(channels, generator=g) * 2 - 1) * bound
     return features, idx, weight, bias
+
+
+# The refinement modules of the three shipped setups: GaussianFormer-1 config/nuscenes_gs25600_solid.py:69-76,133-147
+# and config/nuscenes_gs144000.py:69-76,133-147, GaussianFormer-2 config/prob/nuscenes_gs25600.py:87-94,116,183-194
+# (19 200 lifted anchors + 6 400 random ones).  The anchor has the refined row's layout, so anchor_dim = out_dim.
+REFINE_CONFIGS = {
+    "gs25600_solid": dict(variant="v1", num_anchor=25600, unit_xyz=(4.0, 4.0, 1.0), refine_manual=[0, 1, 2],
+                          restrict_xyz=True, semantics_activation="softplus", semantic_dim=17, include_opa=True,
+                          pc_range=(-50.0, -50.0, -5.0, 50.0, 50.0, 3.0), scale_range=(0.08, 0.64)),
+    "gs144000": dict(variant="v1", num_anchor=144000, unit_xyz=(2.0, 2.0, 0.5), refine_manual=[0, 1, 2],
+                     restrict_xyz=True, semantics_activation="identity", semantic_dim=18, include_opa=False,
+                     pc_range=(-50.0, -50.0, -5.0, 50.0, 50.0, 3.0), scale_range=(0.08, 0.32)),
+    "prob_gs25600": dict(variant="v2", num_anchor=19200 + 6400, unit_xyz=(4.0, 4.0, 1.0), refine_manual=None,
+                         restrict_xyz=False, semantics_activation="identity", semantic_dim=17, include_opa=True,
+                         pc_range=(-50.0, -50.0, -5.0, 50.0, 50.0, 3.0), scale_range=(0.01, 1.8)),
+}
+# Shares of the drawn inputs that exercise the clamps (assumptions, not statistics of a trained model): anchors near a
+# pc-range face with a delta that pushes them past it, xyz / scale / opacity logits beyond +-9.21, and semantic logits
+# around the softplus threshold.
+REFINE_FACE_SHARE, REFINE_BEYOND_SHARE, REFINE_HIGH_SEM_SHARE = 0.05, 0.02, 0.02
+
+
+def _refine_clamp_inputs(out, anchor, cfg):
+    """The fp64 values of the refinement that meet a clamp or the softplus threshold, as (value, bound) pairs, for the
+    margin test of make_refine_inputs."""
+    o, a = out.double(), anchor.double()
+    lo = torch.tensor(cfg["pc_range"][:3], dtype=torch.float64)
+    ext = torch.tensor(cfg["pc_range"][3:], dtype=torch.float64) - lo
+    sig = lambda v: torch.sigmoid(v.clamp(-9.21, 9.21))                                 # noqa: E731
+    unit = torch.tensor(cfg["unit_xyz"], dtype=torch.float64)
+    opa = int(cfg["include_opa"])
+    pairs = [(o[..., 0:6], 9.21), (o[..., 10:10 + opa], 9.21)]
+    if cfg["variant"] == "v1":
+        x = (2 * sig(o[..., :3]) - 1) * (4 * unit / ext) + a[..., :3]
+        pairs.append((x, 9.21))
+    else:
+        t = (sig(a[..., :3]) * ext + lo + (2 * sig(o[..., :3]) - 1) * unit - lo) / ext
+        pairs += [(a[..., :3], 9.21), (t, 1e-4), (t, 0.9999)]
+    if cfg["semantics_activation"] == "softplus":
+        pairs.append((o[..., 10 + opa:], 20.0))
+    return pairs
+
+
+def make_refine_inputs(config="gs25600_solid", batch=1, num_anchor=None, embed_dims=128, seed=0, margin=False):
+    """Inputs of ``ops.gaussian_refine`` / the refinement modules for one of ``REFINE_CONFIGS``: the MLP output ``out``
+    ``[B, A, D]`` and the incoming ``anchor`` ``[B, A, D]`` (fp32, on the CPU), with ``instance_feature`` and
+    ``anchor_embed`` ``[B, A, embed_dims]`` for the whole module.
+
+    Anchors: xyz logits of a position in pc_range (GaussianFormer-2: the first 3/4 near the ground, z in the lower
+    half, the rest uniform), N(0, 1) scale logits, an un-normalised N(0, 1) quaternion, N(0, 1) opacity and semantics.
+    ``out``: N(0, 1.5) xyz logits, N(0, 1) for the rest, semantics N(0, 3).  On top, ``REFINE_FACE_SHARE`` of the
+    anchors sit within 1e-3 of a pc-range face on one axis (xyz logit beyond +-6.9) with an xyz logit in ``out`` that
+    pushes them outward, so that V1's means and V2's inverse sigmoid meet their clamps; ``REFINE_BEYOND_SHARE`` of the
+    xyz, scale and opacity logits are U(+-(9.21, 12)); ``REFINE_HIGH_SEM_SHARE`` of the semantic logits are U(15, 25).
+
+    ``margin=True`` re-draws every anchor one of whose values meets a clamp (+-9.21f, V2's 1e-4 and 0.9999) or the
+    softplus threshold within 1e-3, so that an fp32 evaluation decides every clamp as the fp64 one does.  The
+    saturated inverse sigmoid is log(0.9999 / 1e-4) = 9.21024, beyond the sigmoid's 9.21 by construction; its gradient
+    is 0 either way.  Returns a dict with those tensors and the module's constructor arguments under ``config``."""
+    cfg = REFINE_CONFIGS[config]
+    A = cfg["num_anchor"] if num_anchor is None else num_anchor
+    opa, S = int(cfg["include_opa"]), cfg["semantic_dim"]
+    D = 10 + opa + S
+    gen = torch.Generator().manual_seed(seed)
+
+    def draw(n):
+        u = torch.rand(n, 3, generator=gen) * 0.96 + 0.02
+        if cfg["variant"] == "v2":
+            lifted = torch.arange(n) % 4 != 3                                  # 19 200 of 25 600
+            u[lifted, 2] = u[lifted, 2] * 0.5
+        anchor = torch.cat([torch.log(u / (1 - u)), torch.randn(n, D - 3, generator=gen)], -1)
+        out = torch.cat([torch.randn(n, 3, generator=gen) * 1.5, torch.randn(n, 7 + opa, generator=gen),
+                         torch.randn(n, S, generator=gen) * 3.0], -1)
+        face = torch.rand(n, generator=gen) < REFINE_FACE_SHARE
+        nf = int(face.sum())
+        axis = torch.randint(0, 3, (nf,), generator=gen)
+        side = torch.where(torch.rand(nf, generator=gen) < 0.5, -1.0, 1.0)
+        rows = face.nonzero()[:, 0]
+        anchor[rows, axis] = side * (6.9 + 2.2 * torch.rand(nf, generator=gen))
+        out[rows, axis] = side * (1.0 + 2.0 * torch.rand(nf, generator=gen))
+        cols = torch.cat([torch.arange(6), torch.arange(10, 10 + opa)])        # the clamped logits of out
+        beyond = torch.rand(n, len(cols), generator=gen) < REFINE_BEYOND_SHARE
+        mag = (9.21 + 2.79 * torch.rand(n, len(cols), generator=gen)) * torch.where(
+            torch.rand(n, len(cols), generator=gen) < 0.5, -1.0, 1.0)
+        out[:, cols] = torch.where(beyond, mag, out[:, cols])
+        if S:
+            high = torch.rand(n, S, generator=gen) < REFINE_HIGH_SEM_SHARE
+            out[:, 10 + opa:][high] = 15.0 + 10.0 * torch.rand(int(high.sum()), generator=gen)
+        return out, anchor
+
+    out, anchor = draw(batch * A)
+    if margin:
+        for _ in range(100):
+            bad = torch.zeros(batch * A, dtype=torch.bool)
+            for v, bound in _refine_clamp_inputs(out, anchor, cfg):
+                if v.numel():
+                    bad |= ((v.abs() - bound).abs() < 1e-3).reshape(batch * A, -1).any(-1)
+            if not bad.any():
+                break
+            out[bad], anchor[bad] = draw(int(bad.sum()))
+        else:
+            raise RuntimeError("make_refine_inputs: values near a clamp after 100 re-draws")
+    module = dict(pc_range=list(cfg["pc_range"]), scale_range=list(cfg["scale_range"]),
+                  unit_xyz=list(cfg["unit_xyz"]), semantics=S > 0, semantic_dim=S, include_opa=cfg["include_opa"],
+                  semantics_activation=cfg["semantics_activation"], embed_dims=embed_dims)
+    if cfg["variant"] == "v1":
+        module.update(restrict_xyz=cfg["restrict_xyz"], refine_manual=list(cfg["refine_manual"]))
+    return dict(out=out.reshape(batch, A, D).contiguous(), anchor=anchor.reshape(batch, A, D).contiguous(),
+                instance_feature=torch.randn(batch, A, embed_dims, generator=gen),
+                anchor_embed=torch.randn(batch, A, embed_dims, generator=gen), variant=cfg["variant"], config=module)

@@ -520,6 +520,82 @@ int gf_subm_conv_backward(const gf_subm_conv_desc *desc, void *workspace, const 
                           const float *grad_out, float *grad_features, float *grad_weight, float *grad_bias,
                           gf_stream_t stream);
 
+/* ---- Gaussian refinement: the arithmetic of SparseGaussian3DRefinementModule.forward after its MLP
+ * (model/encoder/gaussian_encoder/refine_module.py:72-123, GF_REFINE_V1) and of SparseGaussian3DRefinementModuleV2
+ * (refine_module_v2.py:64-108, GF_REFINE_V2), with its gradient.  Inputs: out [B, A, D], the MLP output after mmcv's
+ * Scale, D = out_dim = 10 + opa + S (opa = include_opa in {0, 1}, S = semantic_dim), and anchor [B, A, Da].  With the
+ * descriptor's constants (the fp32 values the reference's fp32 tensors are combined with):
+ *
+ *   ssig(v)      = sigmoid(clamp(v, -9.21f, 9.21f))                                                  safe_sigmoid
+ *   sinv(t)      = log(t' / (1 - t')),  t' = clamp(t, (float)(1 - 0.9999), 0.9999f)               safe_inverse_sigmoid
+ *   normalize(q) = q / max(|q|, 1e-12f)                                                             F.normalize
+ *   lo[i] = pc_range[i], extent[i] = (float)(pc_range[i + 3] - pc_range[i])
+ *   act          = softmax (max subtracted) | softplus (beta 1, threshold 20: x itself where x > 20) | identity
+ *
+ * V1 (o = out[b, a], one row):
+ *   restrict_xyz:  o[0:3] = (2 ssig(o[0:3]) - 1) * unit      unit[i] = (float)(4 unit_xyz[i] / extent_i), in double
+ *   o[0:r] += anchor[0:r]                                    r = refine_prefix (refine_manual must be [0, r))
+ *   rot = normalize(o[6:10]);  new_anchor = [o[0:6], rot, o[10:D]]
+ * V2:
+ *   delta = (2 ssig(out[0:3]) - 1) * unit                    unit = unit_xyz in metres, as the fp32 buffer holds it
+ *   orig  = ssig(anchor[0:3]) * extent + lo
+ *   axyz  = sinv((orig + delta - lo) / extent)
+ *   new_anchor = [axyz, out[3:6], rot, out[10:D]],  rot = normalize(out[6:10]);  o = new_anchor
+ * Both:
+ *   means     = ssig(o[0:3]) * extent + lo                   (V2: o[0:3] = axyz)
+ *   scales    = scale_lo + scale_extent * ssig(o[3:6])
+ *   rotations = rot,  opacities = ssig(o[10:10+opa]),  semantics = act(o[10+opa:D])
+ *   V2 only:  original_means = orig,  delta_means = delta
+ *
+ * in fp64 from the fp32 inputs, each output rounded to fp32 once; one thread per anchor.  Shapes: new_anchor [B, A, D],
+ * means, scales, original_means, delta_means [B, A, 3], rotations [B, A, 4], opacities [B, A, opa], semantics
+ * [B, A, S]; every output the variant has is fully overwritten (original_means and delta_means are ignored by V1).
+ *
+ * gf_gaussian_refine_backward recomputes the forward from out and anchor and takes the gradient of any subset of the
+ * outputs: a NULL gradient counts as zero and is not read.  It fully overwrites grad_out [B, A, D] and grad_anchor
+ * [B, A, Da]; grad_anchor is non-zero only in the columns the forward reads (the first r in V1, 0..2 in V2).  The clamps
+ * pass the gradient on [lo, hi], bounds included, and block it outside (torch.clamp's backward); normalize follows
+ * F.normalize, whose norm below 1e-12f is the constant epsilon; softplus follows PyTorch's threshold.  No atomics: the
+ * results are bit-reproducible.  Neither call needs a workspace or synchronises, so both can be captured in a CUDA graph.
+ *
+ * A NULL desc, negative sizes, an unknown variant or activation, include_opa or restrict_xyz outside {0, 1},
+ * out_dim != 10 + include_opa + semantic_dim, a negative refine_prefix or one above min(out_dim, anchor_dim), V2 with
+ * refine_prefix or restrict_xyz set or anchor_dim < 3, and NULL pointers for non-empty work are GF_ERR_INVALID_ARG;
+ * semantic_dim > GF_REFINE_MAX_SEMANTICS (the semantic logits of an anchor are held in registers) and
+ * B * A * max(D, Da) >= 2^31 are GF_ERR_UNSUPPORTED; all before any CUDA call. */
+#define GF_REFINE_V1 0
+#define GF_REFINE_V2 1
+#define GF_REFINE_IDENTITY 0
+#define GF_REFINE_SOFTMAX 1
+#define GF_REFINE_SOFTPLUS 2
+#define GF_REFINE_MAX_SEMANTICS 32
+
+typedef struct gf_refine_desc {
+    int32_t variant;                             /* GF_REFINE_V1 | GF_REFINE_V2 */
+    int32_t batch, num_anchors, out_dim, anchor_dim;
+    int32_t refine_prefix, restrict_xyz;         /* V1 only (0 for V2) */
+    int32_t include_opa, semantic_dim, semantics_act;
+    float lo[3], extent[3], unit[3];
+    float scale_lo, scale_extent;
+} gf_refine_desc;
+
+typedef struct gf_refine_outputs {
+    float *new_anchor, *means, *scales, *rotations, *opacities, *semantics;
+    float *original_means, *delta_means;         /* V2 only */
+} gf_refine_outputs;
+
+/* the gradients of the outputs, each NULL (zero) or shaped as its output */
+typedef struct gf_refine_grads {
+    const float *new_anchor, *means, *scales, *rotations, *opacities, *semantics;
+    const float *original_means, *delta_means;
+} gf_refine_grads;
+
+int gf_gaussian_refine(const gf_refine_desc *desc, const float *out, const float *anchor,
+                       const gf_refine_outputs *outputs, gf_stream_t stream);
+
+int gf_gaussian_refine_backward(const gf_refine_desc *desc, const float *out, const float *anchor,
+                                const gf_refine_grads *grads, float *grad_out, float *grad_anchor, gf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
